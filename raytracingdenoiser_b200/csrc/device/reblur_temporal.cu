@@ -187,23 +187,36 @@ __device__ __forceinline__ float ResolveBilinearCustom1(const CatRomSetup& s, co
     return sum < 0.0001f ? 0.0f : v / sum;
 }
 
-// thin-lens virtual position (Common.hlsli:404-461, NRD_USE_SPECULAR_MOTION_V2 = 1)
-__device__ __forceinline__ f3 GetXvirtual(float hitDist, float curvature, f3 X, f3 Xprev, f3 N, f3 V, float aLog)
+// thin-lens virtual position (Common.hlsli:404-461, NRD_USE_SPECULAR_MOTION_V2 = 1).  The kernel evaluates it for two hit
+// distances: what does not depend on the hit distance is set up once per pixel (the compiler does not merge the two inlined
+// copies of the dominant direction's powf).
+struct XvirtualSetup
 {
-    f4 D = SpecularDominantDirectionLut(N, V, aLog); // aLog: roughness-table entry of the pixel's roughness
-    f3 ray = xyz(D) * hitDist;
+    f4 D;           // dominant direction, .w = dominant factor
+    float magScale; // 1 / (1 + thin-lens term)
+};
+__device__ __forceinline__ XvirtualSetup SetupXvirtual(float curvature, float lengthX, f3 N, f3 V, float aLog)
+{
+    XvirtualSetup s;
+    s.D = SpecularDominantDirectionLut(N, V, aLog); // aLog: roughness-table entry of the pixel's roughness
+    float f = lengthX * (1.0f - fabsf(dot(N, V))) * fmaxf(curvature, 0.0f);
+    s.magScale = 1.0f / (1.0f + f);
+    return s;
+}
+__device__ __forceinline__ f3 GetXvirtual(const XvirtualSetup& s, float hitDist, float curvature, f3 X, f3 Xprev, f3 N, f3 V)
+{
+    f3 ray = xyz(s.D) * hitDist;
     f3 T, B;
     GetBasis(N, T, B);
     float Oz = -dot(N, ray);
     float Ox = dot(T, ray), Oy = dot(B, ray);
     float mag = 1.0f / (2.0f * curvature * Oz - 1.0f);
-    float f = length(X) * (1.0f - fabsf(dot(N, V))) * fmaxf(curvature, 0.0f);
-    mag *= 1.0f / (1.0f + f);
+    mag *= s.magScale;
     float lenI = sqrtf(Ox * Ox + Oy * Oy + Oz * Oz) * fabsf(mag);
     f3 Iw = V * lenI;
     float closeness = saturate(length(Iw) / (hitDist + kEps));
-    f3 origin = lerp3(Xprev, X, closeness * D.w);
-    return origin - Iw * D.w;
+    f3 origin = lerp3(Xprev, X, closeness * s.D.w);
+    return origin - Iw * s.D.w;
 }
 
 __device__ __forceinline__ float EncodingAwareNormalWeight(f3 Ncurr, f3 Nprev, float maxAngle, float curvatureAngle, float thresholdAngle) // Common.hlsli:578-590
@@ -233,14 +246,22 @@ struct TaArgs
     int perf;            // REBLUR_PERFORMANCE_MODE: no CatRom history filters (REBLUR_Config.hlsli:196-202)
 };
 
-// CB = checkerboarded inputs (compiled out of the default kernels)
-template <bool DIFF, bool SPEC, bool CB = false>
+// GENERAL = false: the kernel of the default configuration, the only one compiled with these switches as constants --
+// perspective projection, 2.5D screen-space motion vectors, no checkerboard, no history-confidence / disocclusion-mix inputs,
+// specular pre-pass on, performance mode off.  GENERAL = true reads them from the constants (LaunchTa picks).
+template <bool DIFF, bool SPEC, bool GENERAL = false>
 #ifndef NRD_B200_TA_MIN_BLOCKS
 #define NRD_B200_TA_MIN_BLOCKS 5 // <= 96 registers: 5 x 128 threads per SM instead of 3 (measured 1.7x on this kernel)
 #endif
 __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAccumulationKernel(const __grid_constant__ TaArgs a)
 {
     const ReblurConstants& c = a.c;
+    const float orthoMode = GENERAL ? c.gOrthoMode : 0.0f;
+    const bool worldSpaceMv = GENERAL && c.gMvScale[3] != 0.0f;
+    const bool hasConfidence = GENERAL && c.gHasHistoryConfidence;
+    const bool hasThresholdMix = GENERAL && c.gHasDisocclusionThresholdMix;
+    const bool specPrepass = !GENERAL || c.gSpecPrepassBlurRadius != 0.0f;
+    const bool perf = GENERAL && a.perf;
     const int x = blockIdx.x * 32 + threadIdx.x;
     const int y = a.rowBegin + blockIdx.y * 4 + threadIdx.y;
     const int maxX = c.gRectSizeMinusOne[0], maxY = c.gRectSizeMinusOne[1];
@@ -250,9 +271,9 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     if (viewZ > c.gDenoisingRange) return;
 
     const f2 pixelUv = PixelUv(x, y, c.gRectSizeInv);
-    const f3 Xv = ReconstructViewPosition(pixelUv, c.gFrustum, viewZ, c.gOrthoMode);
+    const f3 Xv = ReconstructViewPosition(pixelUv, c.gFrustum, viewZ, orthoMode);
     const f3 X = PinnedRotate(c.gViewToWorld, Xv);
-    const unsigned checkerboard = CB ? (((unsigned)x ^ (unsigned)y) ^ c.gFrameIndex) & 1u : 0u; // Sequence::CheckerBoard
+    const unsigned checkerboard = GENERAL ? (((unsigned)x ^ (unsigned)y) ^ c.gFrameIndex) & 1u : 0u; // Sequence::CheckerBoard
 
     // 3x3 neighbourhood: averaged normal (2x2 corner), roughness moments, min hit distance for tracking
     f3 Navg = mk3(0.0f);
@@ -270,7 +291,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
             if (i == 1 && j == 2) n01 = g.N;
             if (SPEC)
             {
-                float h = c.gSpecPrepassBlurRadius == 0.0f ? LoadRGBA16F(Near(a.inSpec), px, py).w : LoadR16F(Near(a.inHitDist), px, py);
+                float h = !specPrepass ? LoadRGBA16F(Near(a.inSpec), px, py).w : LoadR16F(Near(a.inHitDist), px, py);
                 hitDistForTracking = fminf(hitDistForTracking, h == 0.0f ? kInf : h);
                 float r2 = g.roughness * g.roughness;
                 roughnessM1 += r2;
@@ -296,7 +317,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         rng.Initialize(x, y, c.gFrameIndex);
         hitDistForTracking = hitDistForTracking == kInf ? 0.0f : hitDistForTracking;
         hitDistNormalization = (c.gHitDistParams[0] + viewZ * c.gHitDistParams[1]) * g0.hitK;
-        hitDistForTracking *= c.gSpecPrepassBlurRadius == 0.0f ? hitDistNormalization : 1.0f;
+        hitDistForTracking *= !specPrepass ? hitDistNormalization : 1.0f;
         StoreR16F(a.outHitDist, x, y, hitDistForTracking);
     }
 
@@ -306,11 +327,11 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     f3 Xprev = X;
     f2 smbPixelUv = mk2(__fadd_rn(pixelUv.x, mv.x), __fadd_rn(pixelUv.y, mv.y));
     const f3 camDelta = mk3(c.gCameraDelta[0], c.gCameraDelta[1], c.gCameraDelta[2]);
-    if (c.gMvScale[3] == 0.0f)
+    if (!worldSpaceMv)
     {
         if (c.gMvScale[2] == 0.0f) mv.z = __fadd_rn(PinnedRow(c.gWorldToViewPrev, 2, X.x, X.y, X.z), -viewZ);
         float viewZprev = __fadd_rn(viewZ, mv.z);
-        f3 Xvprevlocal = ReconstructViewPosition(smbPixelUv, c.gFrustumPrev, viewZprev, c.gOrthoMode);
+        f3 Xvprevlocal = ReconstructViewPosition(smbPixelUv, c.gFrustumPrev, viewZprev, orthoMode);
         f3 r = PinnedRotateInverse(c.gWorldToViewPrev, Xvprevlocal);
         Xprev = mk3(__fadd_rn(r.x, camDelta.x), __fadd_rn(r.y, camDelta.y), __fadd_rn(r.z, camDelta.z));
     }
@@ -320,42 +341,62 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         smbPixelUv = GetScreenUv(c.gWorldToClipPrev, Xprev);
     }
 
-    // previous viewZ / internal data in the 4x4 CatRom footprint (12 texels, corners unused) around the bilinear origin b
+    // previous viewZ / internal data in the 4x4 CatRom footprint (12 texels, corners unused) around the bilinear origin b.
+    // A texel is occluded when its plane distance exceeds the threshold of its quadrant, and the thresholds need the previous
+    // normal of the inner 2x2 first.  The 8 outer texels only decide whether all 12 pass (CatRom allowed), so they are reduced as
+    // they are loaded: per quadrant the largest plane distance, plus one flag that is cleared by a material mismatch or a NaN
+    // distance (NaN fails `d <= thr`, fmaxf would drop it).  `max <= thr` is then exactly `d <= thr` for both texels.
     const Bilinear smbF = GetBilinear(smbPixelUv, c.gRectSizePrev);
     const int bx = (int)smbF.ox, by = (int)smbF.oy;
     const int W1 = a.prevZ.w - 1, H1 = a.prevZ.h - 1;
-    // index [row][col] with row/col in 0..3 <-> texel (bx - 1 + col, by - 1 + row)
-    float pz[4][4];
-    unsigned pid[4][4];
-    const bool smbLocal = FootprintLocal(a.prevZ, by - 1, by + 2); // one owner test for the 28 loads of this footprint
-    auto gatherSmb = [&](const Surf& prevZ, const Surf& prevInternal) {
+    const float XvprevZ = PinnedRow(c.gWorldToViewPrev, 2, Xprev.x, Xprev.y, Xprev.z);
+    const float minMaterial = fminf(c.gSpecMinMaterial, c.gDiffMinMaterial);
+    const float centerMat = fmaxf(materialID, minMaterial);
+    // inner 2x2, index [row * 2 + col] <-> texel (bx + col, by + row), i.e. gather order 00, 10, 01, 11
+    float pz[4];
+    unsigned pid[4];
+    float outerDist[4] = {0.0f, 0.0f, 0.0f, 0.0f}; // per quadrant, same order
+    bool outerPass = true;
+    // prevZ and prevInternal are full-resolution pool surfaces of one geometry: one row lookup serves both
 #pragma unroll
-        for (int r = 0; r < 4; r++)
+    for (int r = 0; r < 4; r++)
+    {
+        const RowRef row = RefRow(a.prevZ, clampi(by - 1 + r, 0, H1));
 #pragma unroll
-            for (int q = 0; q < 4; q++)
+        for (int q = 0; q < 4; q++)
+        {
+            if ((r == 0 || r == 3) && (q == 0 || q == 3)) continue;
+            const int tx = clampi(bx - 1 + q, 0, W1);
+            const float z = fabsf(__ldg(TexelAt<float>(a.prevZ, row, tx)) * c.gViewZScale);
+            const unsigned id = __ldg(TexelAt<unsigned short>(a.prevInternal, row, tx));
+            if (r >= 1 && r <= 2 && q >= 1 && q <= 2)
             {
-                if ((r == 0 || r == 3) && (q == 0 || q == 3)) continue;
-                int tx = clampi(bx - 1 + q, 0, W1), ty = clampi(by - 1 + r, 0, H1);
-                pz[r][q] = fabsf(LoadR32F(prevZ, tx, ty) * c.gViewZScale);
-                pid[r][q] = LoadU16(prevInternal, tx, ty);
+                pz[(r - 1) * 2 + q - 1] = z;
+                pid[(r - 1) * 2 + q - 1] = id;
             }
-    };
-    if (smbLocal) gatherSmb(Near(a.prevZ), Near(a.prevInternal));
-    else gatherSmb(a.prevZ, a.prevInternal);
+            else
+            {
+                const float d = fabsf(z - XvprevZ);
+                const int k = (r < 2 ? 0 : 2) + (q < 2 ? 0 : 1);
+                outerDist[k] = fmaxf(outerDist[k], d);
+                outerPass &= d == d && centerMat == fmaxf(UnpackInternalData(id).z, minMaterial);
+            }
+        }
+    }
 
     // previous normal averaged over the valid part of the 2x2 footprint
     f3 smbNavg;
     {
         int px = (int)fmaxf(smbF.ox, 0.0f), py = (int)fmaxf(smbF.oy, 0.0f); // uint2(origin): float -> uint saturates at 0
-        float w00 = pz[1][1] < c.gDenoisingRange ? 1.0f : 0.0f, w10 = pz[1][2] < c.gDenoisingRange ? 1.0f : 0.0f;
-        float w01 = pz[2][1] < c.gDenoisingRange ? 1.0f : 0.0f, w11 = pz[2][2] < c.gDenoisingRange ? 1.0f : 0.0f;
+        float w00 = pz[0] < c.gDenoisingRange ? 1.0f : 0.0f, w10 = pz[1] < c.gDenoisingRange ? 1.0f : 0.0f;
+        float w01 = pz[2] < c.gDenoisingRange ? 1.0f : 0.0f, w11 = pz[3] < c.gDenoisingRange ? 1.0f : 0.0f;
         auto sumN = [&](const Surf& prevNr) {
             f3 t = DecodeGuide(LoadPackedNrOrZero(prevNr, px, py)).N * w00;
             t = t + DecodeGuide(LoadPackedNrOrZero(prevNr, px + 1, py)).N * w10;
             t = t + DecodeGuide(LoadPackedNrOrZero(prevNr, px, py + 1)).N * w01;
             return t + DecodeGuide(LoadPackedNrOrZero(prevNr, px + 1, py + 1)).N * w11;
         };
-        f3 s = smbLocal ? sumN(Near(a.prevNr)) : sumN(a.prevNr);
+        f3 s = FootprintLocal(a.prevNr, py, py + 1) ? sumN(Near(a.prevNr)) : sumN(a.prevNr);
         float sum = w00 + w10 + w01 + w11;
         smbNavg = Rotate(c.gWorldPrevToWorld, s * (1.0f / (sum == 0.0f ? 1.0f : sum)));
     }
@@ -363,23 +404,23 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     // parallax in pixels (both definitions, Common.hlsli:319-332)
     const f2 rectSize = mk2(c.gRectSize[0], c.gRectSize[1]);
     const f2 uvPrevOfXprevPlusDelta = GetScreenUv(c.gWorldToClipPrev, Xprev + camDelta);
-    f2 d1 = (uvPrevOfXprevPlusDelta - (c.gOrthoMode == 0.0f ? smbPixelUv : pixelUv)) * rectSize;
-    f2 d2 = (GetScreenUv(c.gWorldToClip, Xprev - camDelta) - (c.gOrthoMode == 0.0f ? pixelUv : smbPixelUv)) * rectSize;
+    f2 d1 = (uvPrevOfXprevPlusDelta - (orthoMode == 0.0f ? smbPixelUv : pixelUv)) * rectSize;
+    f2 d2 = (GetScreenUv(c.gWorldToClip, Xprev - camDelta) - (orthoMode == 0.0f ? pixelUv : smbPixelUv)) * rectSize;
     const float smbParallaxInPixels1 = length(d1), smbParallaxInPixels2 = length(d2);
     const float smbParallaxInPixelsMax = fmaxf(smbParallaxInPixels1, smbParallaxInPixels2);
     const float smbParallaxInPixelsMin = fminf(smbParallaxInPixels1, smbParallaxInPixels2);
 
     // disocclusion threshold
-    const float pixelSize = c.gUnproject * lerpf(viewZ, 1.0f, fabsf(c.gOrthoMode));
-    const float frustumSize = c.gMinRectDimMulUnproject * lerpf(viewZ, 1.0f, fabsf(c.gOrthoMode));
+    const float pixelSize = c.gUnproject * lerpf(viewZ, 1.0f, fabsf(orthoMode));
+    const float frustumSize = c.gMinRectDimMulUnproject * lerpf(viewZ, 1.0f, fabsf(orthoMode));
     float disocclusionThresholdMix = 0.0f;
     if (materialID == c.gStrandMaterialID) disocclusionThresholdMix = pixelSize / (pixelSize + c.gStrandThickness);
-    if (c.gHasDisocclusionThresholdMix) disocclusionThresholdMix = LoadR8Unorm(Near(a.mix), x, y);
+    if (hasThresholdMix) disocclusionThresholdMix = LoadR8Unorm(Near(a.mix), x, y);
     float disocclusionThreshold = lerpf(c.gDisocclusionThreshold, c.gDisocclusionThresholdAlternate, disocclusionThresholdMix);
     const float smallParallax = LinearStep(0.25f, 0.0f, smbParallaxInPixelsMax);
     disocclusionThreshold += 0.05f * smallParallax;
 
-    const f3 V = c.gOrthoMode == 0.0f ? normalize(-X) : mk3(c.gViewVectorWorld[0], c.gViewVectorWorld[1], c.gViewVectorWorld[2]);
+    const f3 V = orthoMode == 0.0f ? normalize(-X) : mk3(c.gViewVectorWorld[0], c.gViewVectorWorld[1], c.gViewVectorWorld[2]);
     const float NoV = fabsf(dot(N, V));
     const float NoVstrict = lerpf(NoV, 1.0f, saturate(smbParallaxInPixelsMax / 30.0f));
     const float almostZeroAngle = 0.0174524064f; // cos(89 deg)
@@ -388,37 +429,23 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     const f4 inScreen = InScreenBilinear(smbF, c.gRectSizePrev);
     const f4 smbThr = mk4(thrBase * inScreen.x - kEps, thrBase * inScreen.y - kEps, thrBase * inScreen.z - kEps, thrBase * inScreen.w - kEps);
 
-    // per-texel occlusion: plane distance against the quadrant's threshold, then material ID
-    const float XvprevZ = PinnedRow(c.gWorldToViewPrev, 2, Xprev.x, Xprev.y, Xprev.z);
-    const float minMaterial = fminf(c.gSpecMinMaterial, c.gDiffMinMaterial);
-    const float centerMat = fmaxf(materialID, minMaterial);
-    float occ[4][4];
-    float occSum = 0.0f;
-#pragma unroll
-    for (int r = 0; r < 4; r++)
-#pragma unroll
-        for (int q = 0; q < 4; q++)
-        {
-            if ((r == 0 || r == 3) && (q == 0 || q == 3)) continue;
-            // quadrant (gather 0..3) of this texel decides which of the four thresholds applies
-            float thr = r < 2 ? (q < 2 ? smbThr.x : smbThr.y) : (q < 2 ? smbThr.z : smbThr.w);
-            float o = fabsf(pz[r][q] - XvprevZ) <= thr ? 1.0f : 0.0f;
-            float m = UnpackInternalData(pid[r][q]).z;
-            o *= centerMat == fmaxf(m, minMaterial) ? 1.0f : 0.0f;
-            occ[r][q] = o;
-            occSum += o;
-        }
-    const f4 smbOcclusion = mk4(occ[1][1], occ[1][2], occ[2][1], occ[2][2]);
+    // occlusion of the inner texels: plane distance against the quadrant's threshold, then material ID
+    auto innerOcclusion = [&](int k, float thr) {
+        float o = fabsf(pz[k] - XvprevZ) <= thr ? 1.0f : 0.0f;
+        return o * (centerMat == fmaxf(UnpackInternalData(pid[k]).z, minMaterial) ? 1.0f : 0.0f);
+    };
+    const f4 smbOcclusion = mk4(innerOcclusion(0, smbThr.x), innerOcclusion(1, smbThr.y), innerOcclusion(2, smbThr.z), innerOcclusion(3, smbThr.w));
     const f4 smbOcclusionWeights = CustomWeights(smbF, smbOcclusion);
-    const bool smbAllowCatRom = occSum > 11.5f && !a.perf;
+    const bool outerAll = outerPass && outerDist[0] <= smbThr.x && outerDist[1] <= smbThr.y && outerDist[2] <= smbThr.z && outerDist[3] <= smbThr.w;
+    const bool smbAllowCatRom = smbOcclusion.x + smbOcclusion.y + smbOcclusion.z + smbOcclusion.w > 3.5f && outerAll && !perf;
     float fbits = smbOcclusion.x + smbOcclusion.y * 2.0f + smbOcclusion.z * 4.0f + smbOcclusion.w * 8.0f;
 
-    const f3 id00 = UnpackInternalData(pid[1][1]), id10 = UnpackInternalData(pid[1][2]), id01 = UnpackInternalData(pid[2][1]), id11 = UnpackInternalData(pid[2][2]);
+    const f3 id00 = UnpackInternalData(pid[0]), id10 = UnpackInternalData(pid[1]), id01 = UnpackInternalData(pid[2]), id11 = UnpackInternalData(pid[3]);
     float diffAccumSpeed = ApplyCustomWeights(id00.x, id10.x, id01.x, id11.x, smbOcclusionWeights);
     float smbSpecAccumSpeed = ApplyCustomWeights(id00.y, id10.y, id01.y, id11.y, smbOcclusionWeights);
 
     // footprint quality
-    const f3 smbVprev = c.gOrthoMode == 0.0f ? normalize(camDelta - Xprev) : mk3(c.gViewVectorWorldPrev[0], c.gViewVectorWorldPrev[1], c.gViewVectorWorldPrev[2]);
+    const f3 smbVprev = orthoMode == 0.0f ? normalize(camDelta - Xprev) : mk3(c.gViewVectorWorldPrev[0], c.gViewVectorWorldPrev[1], c.gViewVectorWorldPrev[2]);
     const float NoVprev = fabsf(dot(N, smbVprev));
     float sizeQuality = (NoVprev + 1e-3f) / (NoV + 1e-3f);
     sizeQuality *= sizeQuality;
@@ -431,14 +458,14 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     if (SPEC)
     {
         float specHistoryConfidence = smbFootprintQuality;
-        if (c.gHasHistoryConfidence) specHistoryConfidence *= LoadR8Unorm(Near(a.specConfidence), x, y);
+        if (hasConfidence) specHistoryConfidence *= LoadR8Unorm(Near(a.specConfidence), x, y);
         smbSpecAccumSpeed *= lerpf(specHistoryConfidence, 1.0f, 1.0f / (1.0f + smbSpecAccumSpeed));
         smbSpecAccumSpeed = fminf(smbSpecAccumSpeed, c.gMaxAccumulatedFrameNum);
         const f4 spec = LoadRGBA16F(Near(a.inSpec), x, y);
 
         // curvature along the predicted motion (REBLUR_TemporalAccumulation.hlsli:364-447)
         {
-            f2 uvForZeroParallax = c.gOrthoMode == 0.0f ? smbPixelUv : pixelUv;
+            f2 uvForZeroParallax = orthoMode == 0.0f ? smbPixelUv : pixelUv;
             f2 deltaUv = (uvForZeroParallax - uvPrevOfXprevPlusDelta) * rectSize;
             float invP = 1.0f / fmaxf(smbParallaxInPixels1, 1.0f / 256.0f);
             deltaUv = deltaUv * invP;
@@ -446,16 +473,16 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
             f3 x10, x01;
             {
                 f2 uv = mk2(pixelUv.x + c.gRectSizeInv[0], pixelUv.y);
-                f3 xw = Rotate(c.gViewToWorld, ReconstructViewPosition(uv, c.gFrustum, 1.0f, c.gOrthoMode));
-                f3 v = c.gOrthoMode == 0.0f ? normalize(-xw) : mk3(c.gViewVectorWorld[0], c.gViewVectorWorld[1], c.gViewVectorWorld[2]);
-                f3 o = c.gOrthoMode == 0.0f ? mk3(0.0f) : xw;
+                f3 xw = Rotate(c.gViewToWorld, ReconstructViewPosition(uv, c.gFrustum, 1.0f, orthoMode));
+                f3 v = orthoMode == 0.0f ? normalize(-xw) : mk3(c.gViewVectorWorld[0], c.gViewVectorWorld[1], c.gViewVectorWorld[2]);
+                f3 o = orthoMode == 0.0f ? mk3(0.0f) : xw;
                 x10 = o + v * (dot(X - o, N) / dot(N, v));
             }
             {
                 f2 uv = mk2(pixelUv.x, pixelUv.y + c.gRectSizeInv[1]);
-                f3 xw = Rotate(c.gViewToWorld, ReconstructViewPosition(uv, c.gFrustum, 1.0f, c.gOrthoMode));
-                f3 v = c.gOrthoMode == 0.0f ? normalize(-xw) : mk3(c.gViewVectorWorld[0], c.gViewVectorWorld[1], c.gViewVectorWorld[2]);
-                f3 o = c.gOrthoMode == 0.0f ? mk3(0.0f) : xw;
+                f3 xw = Rotate(c.gViewToWorld, ReconstructViewPosition(uv, c.gFrustum, 1.0f, orthoMode));
+                f3 v = orthoMode == 0.0f ? normalize(-xw) : mk3(c.gViewVectorWorld[0], c.gViewVectorWorld[1], c.gViewVectorWorld[2]);
+                f3 o = orthoMode == 0.0f ? mk3(0.0f) : xw;
                 x01 = o + v * (dot(X - o, N) / dot(N, v));
             }
             f2 w = mk2(fabsf(deltaUv.x) + 1.0f / 256.0f, fabsf(deltaUv.y) + 1.0f / 256.0f);
@@ -478,7 +505,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
                 f2 motionUvHigh = mk2(__fmul_rn(__fadd_rn(fx, 0.5f), c.gRectSizeInv[0]), __fmul_rn(__fadd_rn(fy, 0.5f), c.gRectSizeInv[1]));
                 const bool tapLocal = RowsLocal(a.z, iy, iy);
                 float zHigh = fabsf((tapLocal ? LoadR32F(Near(a.z), ix, iy) : LoadR32F(a.z, ix, iy)) * c.gViewZScale);
-                f3 xHigh = Rotate(c.gViewToWorld, ReconstructViewPosition(motionUvHigh, c.gFrustum, zHigh, c.gOrthoMode));
+                f3 xHigh = Rotate(c.gViewToWorld, ReconstructViewPosition(motionUvHigh, c.gFrustum, zHigh, orthoMode));
                 f3 nHigh = DecodeGuide(tapLocal ? LoadU32(Near(a.nr), ix, iy) : LoadU32(a.nr, ix, iy)).N;
                 float zError = fabsf(zHigh - viewZ) / fmaxf(zHigh, viewZ);
                 if (zError < 0.1f)
@@ -492,7 +519,9 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         }
 
         // virtual motion
-        const f3 Xvirtual = GetXvirtual(hitDistForTracking, curvature, X, Xprev, N, V, g0.aLog);
+        const float lengthX = length(X);
+        const XvirtualSetup xs = SetupXvirtual(curvature, lengthX, N, V, g0.aLog);
+        const f3 Xvirtual = GetXvirtual(xs, hitDistForTracking, curvature, X, Xprev, N, V);
         const float XvirtualLength = length(Xvirtual);
         f2 vmbPixelUv = GetScreenUv(c.gWorldToClipPrev, Xvirtual);
         if (materialID == c.gCameraAttachedReflectionMaterialID) vmbPixelUv = smbPixelUv;
@@ -504,17 +533,19 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         // 2x2 footprint fetches (clamped, like Gather with a clamp sampler)
         const int vx0 = clampi(vx, 0, W1), vx1 = clampi(vx + 1, 0, W1), vy0 = clampi(vy, 0, H1), vy1 = clampi(vy + 1, 0, H1);
         f2 rrp = RelaxedRoughnessWeightParams(roughness * roughness, c.gRoughnessFraction, 0.003f);
-        const bool vmbLocal = RowsLocal(a.prevNr, vy0, vy1); // one owner test for the 12 loads of this 2x2 footprint
         unsigned vmbNr[4];
         float vmbZ[4];
         unsigned vmbId[4];
-        auto gatherVmb = [&](const Surf& prevNr, const Surf& prevZ, const Surf& prevInternal) {
-            vmbNr[0] = LoadU32(prevNr, vx0, vy0); vmbNr[1] = LoadU32(prevNr, vx1, vy0); vmbNr[2] = LoadU32(prevNr, vx0, vy1); vmbNr[3] = LoadU32(prevNr, vx1, vy1);
-            vmbZ[0] = LoadR32F(prevZ, vx0, vy0); vmbZ[1] = LoadR32F(prevZ, vx1, vy0); vmbZ[2] = LoadR32F(prevZ, vx0, vy1); vmbZ[3] = LoadR32F(prevZ, vx1, vy1);
-            vmbId[0] = LoadU16(prevInternal, vx0, vy0); vmbId[1] = LoadU16(prevInternal, vx1, vy0); vmbId[2] = LoadU16(prevInternal, vx0, vy1); vmbId[3] = LoadU16(prevInternal, vx1, vy1);
-        };
-        if (vmbLocal) gatherVmb(Near(a.prevNr), Near(a.prevZ), Near(a.prevInternal));
-        else gatherVmb(a.prevNr, a.prevZ, a.prevInternal);
+        {
+            // prevNr, prevZ and prevInternal are full-resolution pool surfaces of one geometry: one lookup per row serves all three
+            const RowRef r0 = RefRow(a.prevNr, vy0), r1 = RefRow(a.prevNr, vy1);
+            vmbNr[0] = __ldg(TexelAt<unsigned>(a.prevNr, r0, vx0)); vmbNr[1] = __ldg(TexelAt<unsigned>(a.prevNr, r0, vx1));
+            vmbNr[2] = __ldg(TexelAt<unsigned>(a.prevNr, r1, vx0)); vmbNr[3] = __ldg(TexelAt<unsigned>(a.prevNr, r1, vx1));
+            vmbZ[0] = __ldg(TexelAt<float>(a.prevZ, r0, vx0)); vmbZ[1] = __ldg(TexelAt<float>(a.prevZ, r0, vx1));
+            vmbZ[2] = __ldg(TexelAt<float>(a.prevZ, r1, vx0)); vmbZ[3] = __ldg(TexelAt<float>(a.prevZ, r1, vx1));
+            vmbId[0] = __ldg(TexelAt<unsigned short>(a.prevInternal, r0, vx0)); vmbId[1] = __ldg(TexelAt<unsigned short>(a.prevInternal, r0, vx1));
+            vmbId[2] = __ldg(TexelAt<unsigned short>(a.prevInternal, r1, vx0)); vmbId[3] = __ldg(TexelAt<unsigned short>(a.prevInternal, r1, vx1));
+        }
         f4 vmbRoughness = mk4(DecodeGuide(vmbNr[0]).roughness, DecodeGuide(vmbNr[1]).roughness, DecodeGuide(vmbNr[2]).roughness, DecodeGuide(vmbNr[3]).roughness);
         const float jf = SmoothStep(1.0f, 0.0f, smbParallaxInPixelsMax);
         f4 roughnessWeight;
@@ -536,7 +567,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         };
         const Guide vmbGuide = stochasticNr(vmbPixelUv);
         const f3 vmbN = Rotate(c.gWorldPrevToWorld, vmbGuide.N);
-        const float Dfactor = SpecularDominantFactorLut(NoV, g0.aLog);
+        const float Dfactor = xs.D.w;
         float virtualHistoryNormalBasedConfidence = 1.0f / (1.0f + 0.5f * Dfactor * saturate(length(N - vmbN) - kNormalEncodingError) * vmbPixelsTraveled);
 
         if (smbFootprintQuality == 0.0f) smbNavg = vmbN;
@@ -554,7 +585,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
             f3 vmbV = RotateInverse(c.gWorldToViewPrev, vmbVv);
             float NoXcurr = dot(N, Xprev - camDelta);
             float nxy = N.x * vmbV.x + N.y * vmbV.y, nz = N.z * vmbV.z;
-            auto planeDist = [&](float z) { return fabsf(nxy * (c.gOrthoMode == 0.0f ? z : c.gOrthoMode) + nz * z - NoXcurr); };
+            auto planeDist = [&](float z) { return fabsf(nxy * (orthoMode == 0.0f ? z : orthoMode) + nz * z - NoXcurr); };
             vmbOcclusion.x = (planeDist(vmbViewZ.x) <= vmbThr.x ? 1.0f : 0.0f) * (roughnessWeight.x >= 0.5f ? 1.0f : 0.0f);
             vmbOcclusion.y = (planeDist(vmbViewZ.y) <= vmbThr.y ? 1.0f : 0.0f) * (roughnessWeight.y >= 0.5f ? 1.0f : 0.0f);
             vmbOcclusion.z = (planeDist(vmbViewZ.z) <= vmbThr.z ? 1.0f : 0.0f) * (roughnessWeight.z >= 0.5f ? 1.0f : 0.0f);
@@ -592,10 +623,10 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         float virtualHistoryParallaxBasedConfidence;
         {
             float hitDistForTrackingPrev = SampleLinear1(a.prevHitDist, vmbPixelUv.x * c.gResolutionScalePrev[0], vmbPixelUv.y * c.gResolutionScalePrev[1]);
-            f3 XvirtualPrev = GetXvirtual(hitDistForTrackingPrev, curvature, X, Xprev, N, V, g0.aLog);
+            f3 XvirtualPrev = GetXvirtual(xs, hitDistForTrackingPrev, curvature, X, Xprev, N, V);
             f2 vmbPixelUvPrev = GetScreenUv(c.gWorldToClipPrev, XvirtualPrev);
             if (materialID == c.gCameraAttachedReflectionMaterialID) vmbPixelUvPrev = smbPixelUv;
-            float pixelSizeAtXvirtual = c.gUnproject * lerpf(XvirtualLength, 1.0f, fabsf(c.gOrthoMode));
+            float pixelSizeAtXvirtual = c.gUnproject * lerpf(XvirtualLength, 1.0f, fabsf(orthoMode));
             float r = (lobeTanHalfAngle + curvatureAngle) * fminf(hitDistForTracking, hitDistForTrackingPrev) / pixelSizeAtXvirtual;
             float d = length((vmbPixelUvPrev - vmbPixelUv) * rectSize);
             r = fmaxf(r, 0.1f);
@@ -633,7 +664,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         const float smcModified = SpecMagicCurve(roughnessModified); // used twice below
         float surfaceHistoryConfidence;
         {
-            float ang = atanf(smbParallaxInPixelsMax * pixelSize / length(X));
+            float ang = atanf(smbParallaxInPixelsMax * pixelSize / lengthX);
             float nonLinearAccumSpeed = 1.0f / (1.0f + smbSpecAccumSpeed);
             float h = lerpf(smbSpecHistory.w, spec.w, nonLinearAccumSpeed) * hitDistNormalization;
             float tana0 = LobeTanHalfAngle(roughnessModified, kLobeVolume);
@@ -678,7 +709,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
 
         float smbNl = 1.0f / (1.0f + smbSpecAccumSpeed), vmbNl = 1.0f / (1.0f + vmbSpecAccumSpeed);
         // checkerboarded input: a pixel whose value was resolved from its neighbours accumulates slower (:731-735)
-        const bool specHasData = !CB || c.gSpecCheckerboard == 2u || checkerboard == c.gSpecCheckerboard;
+        const bool specHasData = !GENERAL || c.gSpecCheckerboard == 2u || checkerboard == c.gSpecCheckerboard;
         if (!specHasData)
         {
             smbNl *= lerpf(1.0f - c.gCheckerboardResolveAccumSpeed, 1.0f, smbNl);
@@ -724,7 +755,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     if (DIFF)
     {
         float diffHistoryConfidence = smbFootprintQuality;
-        if (c.gHasHistoryConfidence) diffHistoryConfidence *= LoadR8Unorm(Near(a.diffConfidence), x, y);
+        if (hasConfidence) diffHistoryConfidence *= LoadR8Unorm(Near(a.diffConfidence), x, y);
         diffAccumSpeed *= lerpf(diffHistoryConfidence, 1.0f, 1.0f / (1.0f + diffAccumSpeed));
         diffAccumSpeed = fminf(diffAccumSpeed, c.gMaxAccumulatedFrameNum);
         const f4 diff = LoadRGBA16F(Near(a.inDiff), x, y);
@@ -734,7 +765,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
         const float smbDiffFastHistory = ResolveBilinearCustom1(smbSetup, a.histDiffFast, smbOcclusionWeights);
 
         float nl = 1.0f / (1.0f + diffAccumSpeed);
-        const bool diffHasData = !CB || c.gDiffCheckerboard == 2u || checkerboard == c.gDiffCheckerboard;
+        const bool diffHasData = !GENERAL || c.gDiffCheckerboard == 2u || checkerboard == c.gDiffCheckerboard;
         if (!diffHasData) nl *= lerpf(1.0f - c.gCheckerboardResolveAccumSpeed, 1.0f, nl);
         const float minHitNl = 1.0f / (1.0f + 0.5f * __ldg(&a.lut[1023]).x * c.gMaxAccumulatedFrameNum); // SpecMagicCurve(1)
         f4 diffResult = lerp4(smbDiffHistory, diff, nl);
@@ -1289,7 +1320,7 @@ __global__ void __launch_bounds__(256)
         if (c.gSpecPrepassBlurRadius != 0.0f) hitDistForTracking = fminf(hitDistForTracking, LoadR16F(Near(a.hitDist), x, y));
 
         const f3 V = c.gOrthoMode == 0.0f ? normalize(-X) : mk3(c.gViewVectorWorld[0], c.gViewVectorWorld[1], c.gViewVectorWorld[2]);
-        const f3 Xvirtual = GetXvirtual(hitDistForTracking, curvature, X, Xprev, g0.N, V, g0.aLog);
+        const f3 Xvirtual = GetXvirtual(SetupXvirtual(curvature, length(X), g0.N, V, g0.aLog), hitDistForTracking, curvature, X, Xprev, g0.N, V);
         f2 vmbPixelUv = GetScreenUv(c.gWorldToClipPrev, Xvirtual);
         if (g0.materialID == c.gCameraAttachedReflectionMaterialID) vmbPixelUv = pixelUv;
 
@@ -1397,9 +1428,12 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchTa(const PassLaunch& p)
     a.perf = p.performanceMode ? 1 : 0;
     const int W = (int)a.c.gRectSize[0];
     dim3 grid((W + 31) / 32, (p.rowEnd - p.rowBegin + 3) / 4), block(32, 4);
-    const bool checkerboard = (DIFF && a.c.gDiffCheckerboard != 2u) || (SPEC && a.c.gSpecCheckerboard != 2u);
-    if (checkerboard || p.preloadOnly) NRD_B200_LAUNCH(p, grid, block, a, ReblurTemporalAccumulationKernel<DIFF, SPEC, true>);
-    if (!checkerboard || p.preloadOnly) NRD_B200_LAUNCH(p, grid, block, a, ReblurTemporalAccumulationKernel<DIFF, SPEC>);
+    // the switches ReblurTemporalAccumulationKernel<DIFF, SPEC> compiles as constants
+    const ReblurConstants& c = a.c;
+    const bool isDefault = !(DIFF && c.gDiffCheckerboard != 2u) && !(SPEC && c.gSpecCheckerboard != 2u) && c.gOrthoMode == 0.0f && c.gMvScale[3] == 0.0f &&
+                           !c.gHasHistoryConfidence && !c.gHasDisocclusionThresholdMix && !(SPEC && c.gSpecPrepassBlurRadius == 0.0f) && !a.perf;
+    if (!isDefault || p.preloadOnly) NRD_B200_LAUNCH(p, grid, block, a, ReblurTemporalAccumulationKernel<DIFF, SPEC, true>);
+    if (isDefault || p.preloadOnly) NRD_B200_LAUNCH(p, grid, block, a, ReblurTemporalAccumulationKernel<DIFF, SPEC>);
     return cudaGetLastError();
 }
 cudaError_t LaunchReblurTemporalAccumulation(const PassLaunch& p, int signal)
