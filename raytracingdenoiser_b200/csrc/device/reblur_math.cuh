@@ -98,6 +98,26 @@ __device__ __forceinline__ float PositiveRcp(float x) { return 1.0f / fmaxf(x, 1
 __device__ __forceinline__ float AcosApprox(float x) { return 1.41421356f * sqrtf(OneMinusSat(x)); }
 __device__ __forceinline__ float Pow5(float x) { float t = OneMinusSat(x); float t2 = t * t; return t2 * t2 * t; } // pow(saturate(1-x),5)
 __device__ __forceinline__ float GetStdDev(float m1, float m2) { return sqrtf(fabsf(m2 - m1 * m1)); }
+// floor(x) for |x| < 2^22 without the conversion pipe: x + 1.5 * 2^23 rounded towards -inf has floor(x) in its low mantissa bits.
+// Anything outside that range (inf, NaN, a tap projected from behind the camera) comes out as an index far outside any screen.
+__device__ __forceinline__ float FloorIndex(float x, int& i)
+{
+    const float t = __fadd_rd(x, 12582912.0f);
+    i = __float_as_int(t) - 0x4B400000;
+    return __fadd_rn(t, -12582912.0f);
+}
+
+// Sequence::CheckerBoard (REBLUR_PrePass.hlsli:44): which half of the pixels carries data this frame
+__device__ __forceinline__ unsigned CheckerBoard(int x, int y, unsigned frameIndex) { return (((unsigned)x ^ (unsigned)y) ^ frameIndex) & 1u; }
+// Sequence::Bayer4x4 (frozen: standard 4x4 ordered-dither matrix, see oracle/mathlib.h).  The templates are a codegen pin, not
+// part of the dither: they keep the table out of the units that never call Bayer4x4, because with nvcc 12.9 a table in constant
+// bank 3 moves the strip build's peer table (common.cuh) and changes the code of every strip-build kernel of the unit.
+// Revisit with the next nvcc.
+template <class T = unsigned> static __constant__ T kBayer4x4[16] = {0, 8, 2, 10, 12, 4, 14, 6, 3, 11, 1, 9, 15, 7, 13, 5};
+template <class T = unsigned> __device__ __forceinline__ float Bayer4x4(int x, int y, unsigned frameIndex)
+{
+    return (float)((kBayer4x4<T>[(y & 3) * 4 + (x & 3)] + frameIndex) & 15u) / 16.0f;
+}
 
 // weights: Common.hlsli:547-574 (SmoothStep(1,0,x) == smoothstep01(1 - x))
 __device__ __forceinline__ float NonExpWeight(float x, float px, float py)
@@ -111,6 +131,12 @@ __device__ __forceinline__ float ExpWeight(float x, float px, float py)
     float v = -3.0f * fabsf(x * px + py);
     return __fdividef(1.0f, v * v - v + 1.0f); // a weight in (0, 1]: the 2-ulp reciprocal is enough (the IEEE one costs ~8 instructions per tap)
 }
+__device__ __forceinline__ float EncodingAwareNormalWeight(f3 Ncurr, f3 Nprev, float maxAngle, float curvatureAngle, float thresholdAngle, bool remap = false) // Common.hlsli:578-590
+{
+    float angle = AcosApprox(dot(Ncurr, Nprev));
+    float w = SmoothStep01(1.0f - (angle - curvatureAngle - thresholdAngle) / maxAngle);
+    return remap ? SmoothStep(0.05f, 0.95f, w) : w;
+}
 
 __device__ __forceinline__ float HitDistNormalization(float viewZ, const float* p, float roughness) // NRD.hlsli:520-523
 {
@@ -120,6 +146,13 @@ __device__ __forceinline__ float SpecMagicCurve(float roughness) // Common.hlsli
 {
     float f = 1.0f - exp2f(-200.0f * roughness * roughness);
     return f * sqrtf(sqrtf(saturate(roughness)));
+}
+// Filtering::GetModifiedRoughnessFromNormalVariance (restated in oracle/mathlib.h): avgN is the non-normalised average normal
+__device__ __forceinline__ float ModifiedRoughness(float roughness, f3 avgN)
+{
+    float l = length(avgN);
+    float kappa = saturate(1.0f - l * l) / fmaxf(l * (3.0f - l * l), 1e-15f);
+    return Sqrt01(roughness * roughness + kappa);
 }
 __device__ __forceinline__ float LobeTanHalfAngle(float roughness, float percentOfVolume) // MathLib ImportanceSampling (restated, see oracle/mathlib.h)
 {

@@ -5,48 +5,12 @@
 // disocclusion-mix / base-colour inputs.  Reprojection footprints are selected with pinned arithmetic (common.cuh).
 #include "reblur_math.cuh"
 #include "launch.h"
+#include "samplers.cuh"
 #include "tma.cuh"
 
 namespace nrdb200
 {
 using namespace rb;
-
-// ---------------------------------------------------------------------------------------------
-// software samplers (clamp-to-edge), matching D3D addressing
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ f4 FetchClamped4(const Surf& s, int x, int y) { return LoadRGBA16F(s, clampi(x, 0, s.w - 1), clampi(y, 0, s.h - 1)); }
-__device__ __forceinline__ float FetchClamped1(const Surf& s, int x, int y) { return LoadR16F(s, clampi(x, 0, s.w - 1), clampi(y, 0, s.h - 1)); }
-
-#ifndef NRD_B200_SAMPLER_INLINE
-#define NRD_B200_SAMPLER_INLINE __forceinline__
-#endif
-// rows [ya, yb] after clamping to the texture are local: the footprint can be read through Near(s) (common.cuh)
-__device__ __forceinline__ bool FootprintLocal(const Surf& s, int ya, int yb) { return RowsLocal(s, clampi(ya, 0, s.h - 1), clampi(yb, 0, s.h - 1)); }
-
-__device__ NRD_B200_SAMPLER_INLINE f4 SampleLinear4(const Surf& s, float u, float v)
-{
-    float px = u * (float)s.w - 0.5f, py = v * (float)s.h - 0.5f;
-    float fx = floorf(px), fy = floorf(py);
-    float wx = px - fx, wy = py - fy;
-    int x0 = (int)fx, y0 = (int)fy;
-    f4 a = lerp4(FetchClamped4(s, x0, y0), FetchClamped4(s, x0 + 1, y0), wx);
-    f4 b = lerp4(FetchClamped4(s, x0, y0 + 1), FetchClamped4(s, x0 + 1, y0 + 1), wx);
-    return lerp4(a, b, wy);
-}
-__device__ __forceinline__ float SampleLinear1Impl(const Surf& s, int x0, int y0, float wx, float wy)
-{
-    float a = lerpf(FetchClamped1(s, x0, y0), FetchClamped1(s, x0 + 1, y0), wx);
-    float b = lerpf(FetchClamped1(s, x0, y0 + 1), FetchClamped1(s, x0 + 1, y0 + 1), wx);
-    return lerpf(a, b, wy);
-}
-__device__ __forceinline__ float SampleLinear1(const Surf& s, float u, float v)
-{
-    float px = u * (float)s.w - 0.5f, py = v * (float)s.h - 0.5f;
-    float fx = floorf(px), fy = floorf(py);
-    float wx = px - fx, wy = py - fy;
-    int x0 = (int)fx, y0 = (int)fy;
-    return FootprintLocal(s, y0, y0 + 1) ? SampleLinear1Impl(Near(s), x0, y0, wx, wy) : SampleLinear1Impl(s, x0, y0, wx, wy);
-}
 
 // bilinear footprint: origin = floor(uv * size - 0.5), weights = frac   (pinned)
 struct Bilinear
@@ -85,108 +49,6 @@ __device__ __forceinline__ f4 InScreenBilinear(const Bilinear& f, const float* s
     return mk4(x0 * y0, x1 * y0, x0 * y1, x1 * y1);
 }
 
-// CatRom-12 (no corners) through 5 bilinear taps with fallback to the custom-weight bilinear footprint
-// (Common.hlsli:602-656).  HasFast: additionally resolve a scalar texture with the custom weights (4 loads).
-struct CatRomSetup
-{
-    float u01x, u01y, u01z, u01w, u23x, u23y, u23z, u23w, u4x, u4y;
-    f4 w;
-    float w4, sum;
-    int bx, by;
-    float tcx, tcy; // position of the merged inner taps between texel bx and bx+1 (by and by+1)
-    bool bicubic;
-};
-__device__ __forceinline__ CatRomSetup SetupCatRom(f2 samplePos, const float* invSize, f4 customWeights, bool useBicubic)
-{
-    CatRomSetup s;
-    float cx = floorf(samplePos.x - 0.5f) + 0.5f, cy = floorf(samplePos.y - 0.5f) + 0.5f;
-    float fx = saturate(samplePos.x - cx), fy = saturate(samplePos.y - cy);
-    const float S = 0.5f;
-    float w0x = fx * (fx * (-S * fx + 2.0f * S) - S), w0y = fy * (fy * (-S * fy + 2.0f * S) - S);
-    float w1x = fx * (fx * ((2.0f - S) * fx - (3.0f - S))) + 1.0f, w1y = fy * (fy * ((2.0f - S) * fy - (3.0f - S))) + 1.0f;
-    float w2x = fx * (fx * (-(2.0f - S) * fx + (3.0f - 2.0f * S)) + S), w2y = fy * (fy * (-(2.0f - S) * fy + (3.0f - 2.0f * S)) + S);
-    float w3x = fx * (fx * (S * fx - S)), w3y = fy * (fy * (S * fy - S));
-    float w12x = w1x + w2x, w12y = w1y + w2y;
-    float tcx = w2x / w12x, tcy = w2y / w12y;
-    f4 w = mk4(w12x * w0y, w0x * w12y, w12x * w12y, w3x * w12y);
-    float w4 = w12x * w3y;
-    s.w = useBicubic ? w : customWeights;
-    s.w4 = useBicubic ? w4 : 0.0f;
-    s.sum = s.w.x + s.w.y + s.w.z + s.w.w + s.w4;
-    if (useBicubic)
-    {
-        s.u01x = cx + tcx; s.u01y = cy - 1.0f; s.u01z = cx - 1.0f; s.u01w = cy + tcy;
-        s.u23x = cx + tcx; s.u23y = cy + tcy;  s.u23z = cx + 2.0f; s.u23w = cy + tcy;
-        s.u4x = cx + tcx;  s.u4y = cy + 2.0f;
-    }
-    else
-    {
-        s.u01x = cx;        s.u01y = cy;        s.u01z = cx + 1.0f; s.u01w = cy;
-        s.u23x = cx;        s.u23y = cy + 1.0f; s.u23z = cx + 1.0f; s.u23w = cy + 1.0f;
-        s.u4x = cx + fx;    s.u4y = cy + fy;
-    }
-    s.u01x *= invSize[0]; s.u01y *= invSize[1]; s.u01z *= invSize[0]; s.u01w *= invSize[1];
-    s.u23x *= invSize[0]; s.u23y *= invSize[1]; s.u23z *= invSize[0]; s.u23w *= invSize[1];
-    s.u4x *= invSize[0];  s.u4y *= invSize[1];
-    s.bx = (int)cx;
-    s.by = (int)cy;
-    s.tcx = tcx;
-    s.tcy = tcy;
-    s.bicubic = useBicubic;
-    return s;
-}
-#ifndef NRD_B200_CATROM_INLINE
-#define NRD_B200_CATROM_INLINE __forceinline__
-#endif
-// The reference takes 5 hardware-bilinear taps; a software bilinear tap is 4 loads + 3 lerps, i.e. 20 loads for a
-// footprint of 12 distinct texels.  Here every texel is loaded once and weighted with (tap weight) x (its bilinear weight):
-// the same polynomial, summed in a different order (differences ~1e-6 relative, far inside the parity tolerance).
-// Without a valid bicubic footprint the filter degenerates to the 2x2 texels with the custom bilinear weights.
-template <class LOAD> __device__ __forceinline__ auto ResolveCatRomTexels(const CatRomSetup& s, const Surf& tex, LOAD load) -> decltype(load(tex, 0, 0))
-{
-    typedef decltype(load(tex, 0, 0)) V;
-    const int x0 = s.bx, y0 = s.by;
-    V color;
-    if (s.bicubic)
-    {
-        const float ax = 1.0f - s.tcx, bx = s.tcx, ay = 1.0f - s.tcy, by = s.tcy;
-        color = load(tex, x0, y0 - 1) * (s.w.x * ax) + load(tex, x0 + 1, y0 - 1) * (s.w.x * bx);
-        color = color + load(tex, x0 - 1, y0) * (s.w.y * ay) + load(tex, x0 - 1, y0 + 1) * (s.w.y * by);
-        color = color + load(tex, x0, y0) * (s.w.z * ax * ay) + load(tex, x0 + 1, y0) * (s.w.z * bx * ay);
-        color = color + load(tex, x0, y0 + 1) * (s.w.z * ax * by) + load(tex, x0 + 1, y0 + 1) * (s.w.z * bx * by);
-        color = color + load(tex, x0 + 2, y0) * (s.w.w * ay) + load(tex, x0 + 2, y0 + 1) * (s.w.w * by);
-        color = color + load(tex, x0, y0 + 2) * (s.w4 * ax) + load(tex, x0 + 1, y0 + 2) * (s.w4 * bx);
-    }
-    else
-        color = load(tex, x0, y0) * s.w.x + load(tex, x0 + 1, y0) * s.w.y + load(tex, x0, y0 + 1) * s.w.z + load(tex, x0 + 1, y0 + 1) * s.w.w;
-    return color;
-}
-__device__ NRD_B200_CATROM_INLINE f4 ResolveCatRom4(const CatRomSetup& s, const Surf& tex)
-{
-    auto load = [](const Surf& t, int x, int y) { return FetchClamped4(t, x, y); };
-    f4 color = FootprintLocal(tex, s.by - 1, s.by + 2) ? ResolveCatRomTexels(s, Near(tex), load) : ResolveCatRomTexels(s, tex, load);
-    return s.sum < 0.0001f ? mk4(0.0f) : color * (1.0f / s.sum);
-}
-__device__ __forceinline__ float ResolveCatRom1(const CatRomSetup& s, const Surf& tex)
-{
-    auto load = [](const Surf& t, int x, int y) { return FetchClamped1(t, x, y); };
-    float color = FootprintLocal(tex, s.by - 1, s.by + 2) ? ResolveCatRomTexels(s, Near(tex), load) : ResolveCatRomTexels(s, tex, load);
-    return s.sum < 0.0001f ? 0.0f : color / s.sum;
-}
-// tex.Load(origin + offset) * customWeights, out-of-bounds loads return 0
-__device__ __forceinline__ float LoadOrZero1(const Surf& s, int x, int y) { return Inside(s, x, y) ? LoadR16F(s, x, y) : 0.0f; }
-__device__ __forceinline__ float BilinearCustom1Sum(const CatRomSetup& s, const Surf& tex, f4 cw)
-{
-    return LoadOrZero1(tex, s.bx, s.by) * cw.x + LoadOrZero1(tex, s.bx + 1, s.by) * cw.y + LoadOrZero1(tex, s.bx, s.by + 1) * cw.z +
-           LoadOrZero1(tex, s.bx + 1, s.by + 1) * cw.w;
-}
-__device__ __forceinline__ float ResolveBilinearCustom1(const CatRomSetup& s, const Surf& tex, f4 cw)
-{
-    float v = FootprintLocal(tex, s.by, s.by + 1) ? BilinearCustom1Sum(s, Near(tex), cw) : BilinearCustom1Sum(s, tex, cw);
-    float sum = cw.x + cw.y + cw.z + cw.w;
-    return sum < 0.0001f ? 0.0f : v / sum;
-}
-
 // thin-lens virtual position (Common.hlsli:404-461, NRD_USE_SPECULAR_MOTION_V2 = 1).  The kernel evaluates it for two hit
 // distances: what does not depend on the hit distance is set up once per pixel (the compiler does not merge the two inlined
 // copies of the dominant direction's powf).
@@ -219,16 +81,7 @@ __device__ __forceinline__ f3 GetXvirtual(const XvirtualSetup& s, float hitDist,
     return origin - Iw * s.D.w;
 }
 
-__device__ __forceinline__ float EncodingAwareNormalWeight(f3 Ncurr, f3 Nprev, float maxAngle, float curvatureAngle, float thresholdAngle) // Common.hlsli:578-590
-{
-    float angle = AcosApprox(dot(Ncurr, Nprev));
-    return SmoothStep01(1.0f - (angle - curvatureAngle - thresholdAngle) / maxAngle);
-}
-
 __device__ __forceinline__ unsigned LoadPackedNrOrZero(const Surf& s, int x, int y) { return Inside(s, x, y) ? LoadU32(s, x, y) : 0u; }
-
-// Sequence::Bayer4x4 (frozen: standard 4x4 ordered-dither matrix, see oracle/mathlib.h)
-__constant__ unsigned kBayer4x4[16] = {0, 8, 2, 10, 12, 4, 14, 6, 3, 11, 1, 9, 15, 7, 13, 5};
 
 // =============================================================================================
 // Temporal accumulation
@@ -273,7 +126,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     const f2 pixelUv = PixelUv(x, y, c.gRectSizeInv);
     const f3 Xv = ReconstructViewPosition(pixelUv, c.gFrustum, viewZ, orthoMode);
     const f3 X = PinnedRotate(c.gViewToWorld, Xv);
-    const unsigned checkerboard = GENERAL ? (((unsigned)x ^ (unsigned)y) ^ c.gFrameIndex) & 1u : 0u; // Sequence::CheckerBoard
+    const unsigned checkerboard = GENERAL ? CheckerBoard(x, y, c.gFrameIndex) : 0u;
 
     // 3x3 neighbourhood: averaged normal (2x2 corner), roughness moments, min hit distance for tracking
     f3 Navg = mk3(0.0f);
@@ -308,9 +161,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
     RngHash rng;
     if (SPEC)
     {
-        float l = length(Navg);
-        float kappa = saturate(1.0f - l * l) / fmaxf(l * (3.0f - l * l), 1e-15f);
-        roughnessModified = Sqrt01(roughness * roughness + kappa);
+        roughnessModified = ModifiedRoughness(roughness, Navg);
         roughnessM1 *= 1.0f / 9.0f;
         roughnessM2 *= 1.0f / 9.0f;
         roughnessSigma = GetStdDev(roughnessM1, roughnessM2);
@@ -493,8 +344,7 @@ __global__ void __launch_bounds__(128, NRD_B200_TA_MIN_BLOCKS) ReblurTemporalAcc
 
             // high parallax: replace the 1-pixel edge by a longer one along the motion
             float deltaUvLenFixed = smbParallaxInPixelsMin;
-            float bayerValue = (float)((kBayer4x4[(y & 3) * 4 + (x & 3)] + c.gFrameIndex) & 15u) / 16.0f;
-            deltaUvLenFixed *= 1.0f + c.gFramerateScale * bayerValue;
+            deltaUvLenFixed *= 1.0f + c.gFramerateScale * Bayer4x4(x, y, c.gFrameIndex);
             // pinned: the snapped uv selects a texel
             float mu = __fadd_rn(pixelUv.x, __fmul_rn(__fmul_rn(deltaUvLenFixed, deltaUv.x), c.gRectSizeInv[0]));
             float mvv = __fadd_rn(pixelUv.y, __fmul_rn(__fmul_rn(deltaUvLenFixed, deltaUv.y), c.gRectSizeInv[1]));

@@ -14,7 +14,6 @@ namespace nrdb200
 namespace
 {
 using namespace rb;
-using namespace smp;
 
 constexpr float kNormalUlp = 1.5f / 255.0f;  // RELAX_NORMAL_ULP             RELAX_Config.hlsli
 constexpr float kMaxAccumRelax = 255.0f;     // RELAX_MAX_ACCUM_FRAME_NUM
@@ -22,15 +21,10 @@ constexpr float kAntilagAccelScale = 10.0f;  // RELAX_ANTILAG_ACCELERATION_AMOUN
 constexpr float kCurvatureZThreshold = 0.1f; // NRD_CURVATURE_Z_THRESHOLD
 constexpr float kFp16MaxRx = 65504.0f;
 
-// Poisson.hlsli:40-50 (xy = offset, z = length)
-__constant__ float kPoisson8[8][3] = {{-0.4706069f, -0.4427112f, +0.6461146f}, {-0.9057375f, +0.3003471f, +0.9542373f}, {-0.3487388f, +0.4037880f, +0.5335386f},
-                                      {+0.1023042f, +0.6439373f, +0.6520134f}, {+0.5699277f, +0.3513750f, +0.6695386f}, {+0.2939128f, -0.1131226f, +0.3149309f},
-                                      {+0.7836658f, -0.4208784f, +0.8895339f}, {+0.1564120f, -0.8198990f, +0.8346850f}};
-// GetGaussianWeight(length) = exp(-0.66 length^2) of the eight taps
+// Poisson.hlsli:40-50: offsets of the eight taps and GetGaussianWeight(length) = exp(-0.66 length^2)
 #define NRD_B200_POISSON8_X(i) ((i) == 0 ? -0.4706069f : (i) == 1 ? -0.9057375f : (i) == 2 ? -0.3487388f : (i) == 3 ? 0.1023042f : (i) == 4 ? 0.5699277f : (i) == 5 ? 0.2939128f : (i) == 6 ? 0.7836658f : 0.1564120f)
 #define NRD_B200_POISSON8_Y(i) ((i) == 0 ? -0.4427112f : (i) == 1 ? 0.3003471f : (i) == 2 ? 0.4037880f : (i) == 3 ? 0.6439373f : (i) == 4 ? 0.3513750f : (i) == 5 ? -0.1131226f : (i) == 6 ? -0.4208784f : -0.8198990f)
 #define NRD_B200_POISSON8_GAUSS(i) ((i) == 0 ? 0.7591725f : (i) == 1 ? 0.5482766f : (i) == 2 ? 0.82871586f : (i) == 3 ? 0.75534534f : (i) == 4 ? 0.743887f : (i) == 5 ? 0.9366368f : (i) == 6 ? 0.5931912f : 0.6313964f)
-__constant__ unsigned kBayerRx[16] = {0, 8, 2, 10, 12, 4, 14, 6, 3, 11, 1, 9, 15, 7, 13, 5};
 
 typedef RelaxConstants RC;
 
@@ -51,14 +45,6 @@ __device__ __forceinline__ float LoadR8UnormExactClamped(const Surf& s, int x, i
 // octahedral decode at every tap of every A-trous iteration), roughness / material from the packed bits
 #define RX_GUIDE(a, x, y) rb::LoadGuide((a).guide, (a).nr, x, y)
 __device__ __forceinline__ bool IsSkyTile(const Surf& tiles, int x, int y) { return LoadU8(tiles, x >> 4, y >> 4) != 0; }
-// floor(x) for |x| < 2^22 without the conversion pipe (x + 1.5 * 2^23 rounded towards -inf keeps floor(x) in its low mantissa bits);
-// anything outside that range comes out as an index far outside any screen
-__device__ __forceinline__ float FloorIndexRx(float x, int& i)
-{
-    const float t = __fadd_rd(x, 12582912.0f);
-    i = __float_as_int(t) - 0x4B400000;
-    return __fadd_rn(t, -12582912.0f);
-}
 // signal load of a kernel compiled for one or both signals: the absent signal reads as zero and its arithmetic is dead code
 template <bool PRESENT> __device__ __forceinline__ f4 LoadSignal(const Surf& s, int x, int y) { return PRESENT ? LoadRGBA16F(s, x, y) : mk4(0.0f); }
 
@@ -142,14 +128,7 @@ __device__ __forceinline__ f2 NormalWeightParamsAtrous(float roughness, float fr
     angle = fminf(1.57079632679f, angle);
     return mk2(angle, f);
 }
-__device__ __forceinline__ float SpecularNormalWeightAtrous(f2 p0, f3 n0, f3 n, f3 v0, f3 v) // :147-156
-{
-    float cosa = fminf(dot(n0, n), dot(v0, v));
-    float a = AcosApprox(cosa);
-    a = SmoothStep(0.0f, p0.x, a);
-    return saturate(1.0f - a * p0.y);
-}
-// the same with the sample's view vector given un-normalised (v = -s / |s|): dot(v0, v) = -dot(v0, s) * rsqrt(dot(s, s))
+// :147-156 with the sample's view vector given un-normalised (v = -s / |s|): dot(v0, v) = -dot(v0, s) * rsqrt(dot(s, s))
 __device__ __forceinline__ float SpecularNormalWeightAtrousRaw(f2 p0, f3 n0, f3 n, f3 v0, f3 s)
 {
     float cosa = fminf(dot(n0, n), -dot(v0, s) * rsqrtf(dot(s, s)));
@@ -189,19 +168,6 @@ __device__ __forceinline__ float ParallaxInPixels(f3 X, f2 uv0, const float* m, 
     return sqrtf(dx * dx + dy * dy);
 }
 __device__ __forceinline__ float ThinLens(float O, float curvature) { return O / (2.0f * curvature * O + 1.0f); }
-__device__ __forceinline__ float ModifiedRoughness(float roughness, f3 avgN)
-{
-    float l = length(avgN);
-    float kappa = saturate(1.0f - l * l) / fmaxf(l * (3.0f - l * l), 1e-15f);
-    return Sqrt01(roughness * roughness + kappa);
-}
-__device__ __forceinline__ float EncodingAwareNormalWeightRx(f3 a, f3 b, float maxAngle, float curvatureAngle, float thresholdAngle, bool remap)
-{
-    float angle = AcosApprox(dot(a, b));
-    float w = SmoothStep01(1.0f - (angle - curvatureAngle - thresholdAngle) / maxAngle);
-    if (remap) w = SmoothStep(0.05f, 0.95f, w);
-    return w;
-}
 // thin-lens virtual position (Common.hlsli:404-461)
 __device__ __forceinline__ f3 XvirtualRx(float hitDist, float curvature, f3 X, f3 Xprev, f3 N, f3 V, float roughness)
 {
@@ -369,7 +335,7 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
     float cbW0 = 1.0f, cbW1 = 1.0f, cbMat0 = 0.0f, cbMat1 = 0.0f;
     if (CB)
     {
-        checkerboard = (((unsigned)x ^ (unsigned)y) ^ c.gFrameIndex) & 1u;
+        checkerboard = CheckerBoard(x, y, c.gFrameIndex);
         const int x0 = max(x - 1, 0), x1 = min(x + 1, W - 1);
         const float viewZ0 = UnpackViewZ(c, LoadR32F(a.z, x0, y)), viewZ1 = UnpackViewZ(c, LoadR32F(a.z, x1, y));
         cbMat0 = (float)(LoadU32(a.nr, x0, y) >> 30);
@@ -398,9 +364,9 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
         const float ox = NRD_B200_POISSON8_X(i), oy = NRD_B200_POISSON8_Y(i);
         const float rxv = __fadd_rn(__fmul_rn(ox, rx0), __fmul_rn(oy, rx1)), ryv = __fadd_rn(__fmul_rn(ox, rx2), __fmul_rn(oy, rx3));
         int ix, iy;
-        float fx = FloorIndexRx(__fadd_rn(posX, __fmul_rn(rxv, blurRadius)), ix);
-        const float fy = FloorIndexRx(__fadd_rn(posY, __fmul_rn(ryv, blurRadius)), iy);
-        if (CB && mode != 2u && ((((unsigned)ix ^ (unsigned)iy) ^ c.gFrameIndex) & 1u) != mode)
+        float fx = FloorIndex(__fadd_rn(posX, __fmul_rn(rxv, blurRadius)), ix);
+        const float fy = FloorIndex(__fadd_rn(posY, __fmul_rn(ryv, blurRadius)), iy);
+        if (CB && mode != 2u && CheckerBoard(ix, iy, c.gFrameIndex) != mode)
         {
             const int d = (i & 1) == 0 ? -1 : 1; // ApplyCheckerboardShift: even taps move left, odd taps right
             ix += d;
@@ -673,10 +639,10 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
         const f4 bcw = mk4(tapsValid.x * (omx * omy), tapsValid.y * (bwx * omy), tapsValid.z * (omx * bwy), tapsValid.w * (bwx * bwy));
         const bool useBicubic = bicubicFootprintValid > 0.0f;
         const CatRomSetup cr = SetupCatRom(prevPixelPos, c.gResourceSizeInvPrev, bcw, useBicubic);
-        prevDiffSMB = DIFF ? max4(ResolveCatRom4(cr, a.histDiff), 0.0f) : mk4(0.0f);
-        prevSpecSMB = SPEC ? max4(ResolveCatRom4(cr, a.histSpec), 0.0f) : mk4(0.0f);
-        prevDiffSMBResponsive = DIFF ? xyz(max4(ResolveCatRom4(cr, a.histDiffFast), 0.0f)) : mk3(0.0f);
-        prevSpecSMBResponsive = SPEC ? xyz(max4(ResolveCatRom4(cr, a.histSpecFast), 0.0f)) : mk3(0.0f);
+        prevDiffSMB = DIFF ? max4(ResolveCatRom4<false>(cr, a.histDiff), 0.0f) : mk4(0.0f);
+        prevSpecSMB = SPEC ? max4(ResolveCatRom4<false>(cr, a.histSpec), 0.0f) : mk4(0.0f);
+        prevDiffSMBResponsive = DIFF ? xyz(max4(ResolveCatRom4<false>(cr, a.histDiffFast), 0.0f)) : mk3(0.0f);
+        prevSpecSMBResponsive = SPEC ? xyz(max4(ResolveCatRom4<false>(cr, a.histSpecFast), 0.0f)) : mk3(0.0f);
 
         const float wsum = bcw.x + bcw.y + bcw.z + bcw.w;
         {
@@ -732,7 +698,7 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
         float alpha = SMBReprojectionFound > 0.0f ? fmaxf(1.0f / (diffMaxAccumulatedFrameNum + 1.0f), 1.0f / historyLength) : 1.0f;
         float alphaResponsive = SMBReprojectionFound > 0.0f ? fmaxf(1.0f / (diffMaxFastAccumulatedFrameNum + 1.0f), 1.0f / historyLength) : 1.0f;
         // checkerboarded input: a pixel resolved by the pre-pass accumulates slower (:597-606)
-        if (CB && c.gDiffCheckerboard != 2u && ((((unsigned)x ^ (unsigned)y) ^ c.gFrameIndex) & 1u) != c.gDiffCheckerboard && historyLength > 1.0f)
+        if (CB && c.gDiffCheckerboard != 2u && CheckerBoard(x, y, c.gFrameIndex) != c.gDiffCheckerboard && historyLength > 1.0f)
         {
             alpha *= 1.0f - c.gCheckerboardResolveAccumSpeed;
             alphaResponsive *= 1.0f - c.gCheckerboardResolveAccumSpeed;
@@ -783,8 +749,7 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
         f3 xm = x10 * w.x + x01 * w.y;
         f3 n = normalize(n10 * w.x + n01 * w.y);
         float deltaUvLenFixed = smbParallaxInPixelsMin;
-        float bayer = (float)((kBayerRx[(y & 3) * 4 + (x & 3)] + c.gFrameIndex) & 15u) / 16.0f;
-        deltaUvLenFixed *= 1.0f + c.gFramerateScale * bayer;
+        deltaUvLenFixed *= 1.0f + c.gFramerateScale * Bayer4x4(x, y, c.gFrameIndex);
         // pinned: the snapped uv selects a texel
         float mu = __fadd_rn(pixelUv.x, __fmul_rn(__fmul_rn(deltaUvLenFixed, deltaUv.x), c.gRectSizeInv[0]));
         float mvv = __fadd_rn(pixelUv.y, __fmul_rn(__fmul_rn(deltaUvLenFixed, deltaUv.y), c.gRectSizeInv[1]));
@@ -848,9 +813,9 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
             const f4 bcw = mk4(tv[0] * (omx * omy), tv[1] * (bwx * omy), tv[2] * (omx * bwy), tv[3] * (bwx * bwy));
             const bool useBicubic = SMBReprojectionFound == 2.0f && allValid;
             const CatRomSetup cr = SetupCatRom(prevPixelPos, c.gResourceSizeInvPrev, bcw, useBicubic);
-            prevSpecVMB = max4(ResolveCatRom4(cr, a.histSpec), 0.0f);
-            prevSpecVMBResponsive = max4(ResolveCatRom4(cr, a.histSpecFast), 0.0f);
-            prevReflectionHitTVMB = fmaxf(0.001f, SampleLinear1(a.prevHitDist, prevUVVMB.x * resScalePrev.x, prevUVVMB.y * resScalePrev.y));
+            prevSpecVMB = max4(ResolveCatRom4<false>(cr, a.histSpec), 0.0f);
+            prevSpecVMBResponsive = max4(ResolveCatRom4<false>(cr, a.histSpecFast), 0.0f);
+            prevReflectionHitTVMB = fmaxf(0.001f, SampleLinear1<false>(a.prevHitDist, prevUVVMB.x * resScalePrev.x, prevUVVMB.y * resScalePrev.y));
             f4 pnr = UnpackPrevNormalRoughness(SampleLinearRGBA8(a.prevNr, prevUVVMB.x * resScalePrev.x, prevUVVMB.y * resScalePrev.y));
             prevNormalVMB = Rotate(c.gWorldPrevToWorld, xyz(pnr));
             prevRoughnessVMB = pnr.w;
@@ -870,7 +835,7 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
     const float curvatureAngle = atanf(tanCurvature);
 
     const float lobeHalfAngle = fmaxf(atanf(RelaxLobeTanHalfAngle(currentRoughnessModified)), kNormalUlp);
-    const float normalWeight = EncodingAwareNormalWeightRx(currentNormal, prevNormalVMB, lobeHalfAngle, curvatureAngle, kNormalUlp, true);
+    const float normalWeight = EncodingAwareNormalWeight(currentNormal, prevNormalVMB, lobeHalfAngle, curvatureAngle, kNormalUlp, true);
     virtualHistoryAmount *= lerpf(1.0f - saturate(uvDiffLengthInPixels), 1.0f, normalWeight);
 
     const f2 rrp = RelaxedRoughnessWeightParams(currentRoughness * currentRoughness, c.gRoughnessFraction);
@@ -891,8 +856,8 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
     const f3 bn1 = Rotate(c.gWorldPrevToWorld, xyz(back1)), bn2 = Rotate(c.gWorldPrevToWorld, xyz(back2));
     const bool in1 = backUV1.x > 0.0f && backUV1.y > 0.0f && backUV1.x < 1.0f && backUV1.y < 1.0f;
     const bool in2 = backUV2.x > 0.0f && backUV2.y > 0.0f && backUV2.x < 1.0f && backUV2.y < 1.0f;
-    float prevPrevNormalWeight = in1 ? EncodingAwareNormalWeightRx(prevNormalVMB, bn1, lobeHalfAngle, curvatureAngle * 2.0f, kNormalUlp, true) : 1.0f;
-    prevPrevNormalWeight *= in2 ? EncodingAwareNormalWeightRx(prevNormalVMB, bn2, lobeHalfAngle, curvatureAngle * 3.0f, kNormalUlp, true) : 1.0f;
+    float prevPrevNormalWeight = in1 ? EncodingAwareNormalWeight(prevNormalVMB, bn1, lobeHalfAngle, curvatureAngle * 2.0f, kNormalUlp, true) : 1.0f;
+    prevPrevNormalWeight *= in2 ? EncodingAwareNormalWeight(prevNormalVMB, bn2, lobeHalfAngle, curvatureAngle * 3.0f, kNormalUlp, true) : 1.0f;
     virtualHistoryAmount *= 0.33f + 0.67f * prevPrevNormalWeight;
     specVMBConfidence *= 0.33f + 0.67f * prevPrevNormalWeight;
     float rw = NonExpWeight(back1.w * back1.w, rrp.x, rrp.y);
@@ -930,7 +895,7 @@ template <bool DIFF, bool SPEC, bool CB = false> __global__ void __launch_bounds
     float specSMBAlpha = fmaxf(1.0f - specSMBConfidence, 1.0f / (1.0f + specHistoryFrames));
     float specSMBResponsiveAlpha = fmaxf(specSMBAlpha, 1.0f / (1.0f + specHistoryResponsiveFrames));
     // checkerboarded input (:854-863, :881-887)
-    const bool specResolved = CB && c.gSpecCheckerboard != 2u && ((((unsigned)x ^ (unsigned)y) ^ c.gFrameIndex) & 1u) != c.gSpecCheckerboard && smbParallaxInPixelsMax < 0.5f;
+    const bool specResolved = CB && c.gSpecCheckerboard != 2u && CheckerBoard(x, y, c.gFrameIndex) != c.gSpecCheckerboard && smbParallaxInPixelsMax < 0.5f;
     if (specResolved)
     {
         const float k = 1.0f - c.gCheckerboardResolveAccumSpeed * smbFound;

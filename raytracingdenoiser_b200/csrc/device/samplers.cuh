@@ -1,41 +1,40 @@
 // Software samplers with D3D clamp-to-edge addressing and the CatRom-12 / custom-weight bilinear history filter
-// (Common.hlsli:602-656), shared by the RELAX kernels.
+// (Common.hlsli:602-656), shared by the REBLUR and RELAX temporal passes.
+// In the strip build, with FOOTPRINT_TEST (REBLUR) each footprint takes one FootprintLocal() test and is read through Near()
+// views when all its rows are held locally (common.cuh); without it (RELAX) every load does the owner lookup.  The two forms
+// compute the same sums, but ptxas fuses their multiplies and adds differently, so the form decides the strip build's output
+// bytes: RELAX keeps the per-load form and with it the bytes it has always produced.
 #pragma once
 #include "common.cuh"
 
 namespace nrdb200
 {
-namespace smp
-{
 __device__ __forceinline__ f4 FetchClamped4(const Surf& s, int x, int y) { return LoadRGBA16F(s, clampi(x, 0, s.w - 1), clampi(y, 0, s.h - 1)); }
 __device__ __forceinline__ float FetchClamped1(const Surf& s, int x, int y) { return LoadR16F(s, clampi(x, 0, s.w - 1), clampi(y, 0, s.h - 1)); }
 
-__device__ __forceinline__ f4 SampleLinear4(const Surf& s, float u, float v)
+// rows [ya, yb] after clamping to the texture are local: the footprint can be read through Near(s) (common.cuh)
+__device__ __forceinline__ bool FootprintLocal(const Surf& s, int ya, int yb) { return RowsLocal(s, clampi(ya, 0, s.h - 1), clampi(yb, 0, s.h - 1)); }
+
+__device__ __forceinline__ float SampleLinear1Impl(const Surf& s, int x0, int y0, float wx, float wy)
 {
-    float px = u * (float)s.w - 0.5f, py = v * (float)s.h - 0.5f;
-    float fx = floorf(px), fy = floorf(py);
-    float wx = px - fx, wy = py - fy;
-    int x0 = (int)fx, y0 = (int)fy;
-    f4 a = lerp4(FetchClamped4(s, x0, y0), FetchClamped4(s, x0 + 1, y0), wx);
-    f4 b = lerp4(FetchClamped4(s, x0, y0 + 1), FetchClamped4(s, x0 + 1, y0 + 1), wx);
-    return lerp4(a, b, wy);
-}
-__device__ __forceinline__ float SampleLinear1(const Surf& s, float u, float v)
-{
-    float px = u * (float)s.w - 0.5f, py = v * (float)s.h - 0.5f;
-    float fx = floorf(px), fy = floorf(py);
-    float wx = px - fx, wy = py - fy;
-    int x0 = (int)fx, y0 = (int)fy;
     float a = lerpf(FetchClamped1(s, x0, y0), FetchClamped1(s, x0 + 1, y0), wx);
     float b = lerpf(FetchClamped1(s, x0, y0 + 1), FetchClamped1(s, x0 + 1, y0 + 1), wx);
     return lerpf(a, b, wy);
 }
+template <bool FOOTPRINT_TEST = true> __device__ __forceinline__ float SampleLinear1(const Surf& s, float u, float v)
+{
+    float px = u * (float)s.w - 0.5f, py = v * (float)s.h - 0.5f;
+    float fx = floorf(px), fy = floorf(py);
+    float wx = px - fx, wy = py - fy;
+    int x0 = (int)fx, y0 = (int)fy;
+    return FOOTPRINT_TEST && FootprintLocal(s, y0, y0 + 1) ? SampleLinear1Impl(Near(s), x0, y0, wx, wy) : SampleLinear1Impl(s, x0, y0, wx, wy);
+}
 
-
-// CatRom-12 (no corners) through 5 bilinear taps with fallback to the custom-weight bilinear footprint
-// (Common.hlsli:602-656).  HasFast: additionally resolve a scalar texture with the custom weights (4 loads).
+// CatRom-12 (no corners) with fallback to the custom-weight bilinear footprint (Common.hlsli:602-656)
 struct CatRomSetup
 {
+    // uv of the reference's five bilinear taps.  Nothing reads them: a codegen pin, not part of the filter.  Without them
+    // nvcc 12.9 allocates the registers of the REBLUR temporal kernels differently; revisit with the next nvcc.
     float u01x, u01y, u01z, u01w, u23x, u23y, u23z, u23w, u4x, u4y;
     f4 w;
     float w4, sum;
@@ -82,35 +81,52 @@ __device__ __forceinline__ CatRomSetup SetupCatRom(f2 samplePos, const float* in
     s.bicubic = useBicubic;
     return s;
 }
-// The reference takes 5 hardware-bilinear taps; in software that is 20 texel loads for a footprint of 12 distinct texels.
-// Every texel is loaded once and weighted with (tap weight) x (its bilinear weight): the same polynomial summed in a different
-// order (~1e-6 relative).  Without a valid bicubic footprint: the 2x2 texels with the custom bilinear weights.
-__device__ __forceinline__ f4 ResolveCatRom4(const CatRomSetup& s, const Surf& tex)
+// The reference takes 5 hardware-bilinear taps; a software bilinear tap is 4 loads + 3 lerps, i.e. 20 loads for a
+// footprint of 12 distinct texels.  Here every texel is loaded once and weighted with (tap weight) x (its bilinear weight):
+// the same polynomial, summed in a different order (differences ~1e-6 relative, far inside the parity tolerance).
+// Without a valid bicubic footprint the filter degenerates to the 2x2 texels with the custom bilinear weights.
+template <class LOAD> __device__ __forceinline__ auto ResolveCatRomTexels(const CatRomSetup& s, const Surf& tex, LOAD load) -> decltype(load(tex, 0, 0))
 {
+    typedef decltype(load(tex, 0, 0)) V;
     const int x0 = s.bx, y0 = s.by;
-    f4 color;
+    V color;
     if (s.bicubic)
     {
         const float ax = 1.0f - s.tcx, bx = s.tcx, ay = 1.0f - s.tcy, by = s.tcy;
-        color = FetchClamped4(tex, x0, y0 - 1) * (s.w.x * ax) + FetchClamped4(tex, x0 + 1, y0 - 1) * (s.w.x * bx);
-        color = color + FetchClamped4(tex, x0 - 1, y0) * (s.w.y * ay) + FetchClamped4(tex, x0 - 1, y0 + 1) * (s.w.y * by);
-        color = color + FetchClamped4(tex, x0, y0) * (s.w.z * ax * ay) + FetchClamped4(tex, x0 + 1, y0) * (s.w.z * bx * ay);
-        color = color + FetchClamped4(tex, x0, y0 + 1) * (s.w.z * ax * by) + FetchClamped4(tex, x0 + 1, y0 + 1) * (s.w.z * bx * by);
-        color = color + FetchClamped4(tex, x0 + 2, y0) * (s.w.w * ay) + FetchClamped4(tex, x0 + 2, y0 + 1) * (s.w.w * by);
-        color = color + FetchClamped4(tex, x0, y0 + 2) * (s.w4 * ax) + FetchClamped4(tex, x0 + 1, y0 + 2) * (s.w4 * bx);
+        color = load(tex, x0, y0 - 1) * (s.w.x * ax) + load(tex, x0 + 1, y0 - 1) * (s.w.x * bx);
+        color = color + load(tex, x0 - 1, y0) * (s.w.y * ay) + load(tex, x0 - 1, y0 + 1) * (s.w.y * by);
+        color = color + load(tex, x0, y0) * (s.w.z * ax * ay) + load(tex, x0 + 1, y0) * (s.w.z * bx * ay);
+        color = color + load(tex, x0, y0 + 1) * (s.w.z * ax * by) + load(tex, x0 + 1, y0 + 1) * (s.w.z * bx * by);
+        color = color + load(tex, x0 + 2, y0) * (s.w.w * ay) + load(tex, x0 + 2, y0 + 1) * (s.w.w * by);
+        color = color + load(tex, x0, y0 + 2) * (s.w4 * ax) + load(tex, x0 + 1, y0 + 2) * (s.w4 * bx);
     }
     else
-        color = FetchClamped4(tex, x0, y0) * s.w.x + FetchClamped4(tex, x0 + 1, y0) * s.w.y + FetchClamped4(tex, x0, y0 + 1) * s.w.z + FetchClamped4(tex, x0 + 1, y0 + 1) * s.w.w;
+        color = load(tex, x0, y0) * s.w.x + load(tex, x0 + 1, y0) * s.w.y + load(tex, x0, y0 + 1) * s.w.z + load(tex, x0 + 1, y0 + 1) * s.w.w;
+    return color;
+}
+template <bool FOOTPRINT_TEST = true> __device__ __forceinline__ f4 ResolveCatRom4(const CatRomSetup& s, const Surf& tex)
+{
+    auto load = [](const Surf& t, int x, int y) { return FetchClamped4(t, x, y); };
+    f4 color = FOOTPRINT_TEST && FootprintLocal(tex, s.by - 1, s.by + 2) ? ResolveCatRomTexels(s, Near(tex), load) : ResolveCatRomTexels(s, tex, load);
     return s.sum < 0.0001f ? mk4(0.0f) : color * (1.0f / s.sum);
 }
 __device__ __forceinline__ float ResolveCatRom1(const CatRomSetup& s, const Surf& tex)
 {
-    float color = SampleLinear1(tex, s.u01x, s.u01y) * s.w.x;
-    color += SampleLinear1(tex, s.u01z, s.u01w) * s.w.y;
-    color += SampleLinear1(tex, s.u23x, s.u23y) * s.w.z;
-    color += SampleLinear1(tex, s.u23z, s.u23w) * s.w.w;
-    if (s.w4 != 0.0f) color += SampleLinear1(tex, s.u4x, s.u4y) * s.w4;
+    auto load = [](const Surf& t, int x, int y) { return FetchClamped1(t, x, y); };
+    float color = FootprintLocal(tex, s.by - 1, s.by + 2) ? ResolveCatRomTexels(s, Near(tex), load) : ResolveCatRomTexels(s, tex, load);
     return s.sum < 0.0001f ? 0.0f : color / s.sum;
 }
-} // namespace smp
+// tex.Load(origin + offset) * customWeights, out-of-bounds loads return 0
+__device__ __forceinline__ float LoadOrZero1(const Surf& s, int x, int y) { return Inside(s, x, y) ? LoadR16F(s, x, y) : 0.0f; }
+__device__ __forceinline__ float BilinearCustom1Sum(const CatRomSetup& s, const Surf& tex, f4 cw)
+{
+    return LoadOrZero1(tex, s.bx, s.by) * cw.x + LoadOrZero1(tex, s.bx + 1, s.by) * cw.y + LoadOrZero1(tex, s.bx, s.by + 1) * cw.z +
+           LoadOrZero1(tex, s.bx + 1, s.by + 1) * cw.w;
+}
+__device__ __forceinline__ float ResolveBilinearCustom1(const CatRomSetup& s, const Surf& tex, f4 cw)
+{
+    float v = FootprintLocal(tex, s.by, s.by + 1) ? BilinearCustom1Sum(s, Near(tex), cw) : BilinearCustom1Sum(s, tex, cw);
+    float sum = cw.x + cw.y + cw.z + cw.w;
+    return sum < 0.0001f ? 0.0f : v / sum;
+}
 } // namespace nrdb200

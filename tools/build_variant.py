@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """A/B builds of the product library: recompiles the named kernel translation units with extra nvcc flags and links them with the
 other (unchanged) objects into raytracingdenoiser_b200/libnrd_b200_<name>.so.  Select it at run time with
-NRD_B200_LIB=<path> (raytracingdenoiser_b200/nrd.py).   python tools/build_variant.py u4 reblur_spatial.cu -DNRD_B200_TAP_UNROLL=4"""
+NRD_B200_LIB=<path> (raytracingdenoiser_b200/nrd.py).   python tools/build_variant.py ta4 reblur_temporal.cu -DNRD_B200_TA_MIN_BLOCKS=4"""
 import os
 import subprocess
 import sys

@@ -38,6 +38,36 @@ def gpu_info():
         return {"gpu": "unknown (%s)" % e}
 
 
+class Digests(object):
+    """Byte digests of textures, reduced on the GPU: the sum of the 32-bit words, and two sums weighted by the word index."""
+
+    def __init__(self, ctx, stream):
+        self.ctx, self.stream, self.weights, self.staging = ctx, stream, {}, {}
+
+    def tensor(self, t):
+        import torch
+        v = t.contiguous().view(torch.uint8).reshape(-1).view(torch.int32).to(torch.int64)
+        if v.numel() not in self.weights:
+            i = torch.arange(v.numel(), device=v.device, dtype=torch.int64)
+            self.weights[v.numel()] = ((i % 8191) + 1, (i % 65521) + 1)
+        w1, w2 = self.weights[v.numel()]
+        return torch.stack([v.sum(), (v * w1).sum(), (v * w2).sum()])
+
+    def texture(self, rtype, index):
+        # the texel bytes of the rows the context holds, copied into a buffer of the texture's pitch (padding stays zero)
+        import torch
+        info = self.ctx.get_texture(rtype, index)
+        key = (int(rtype), index)
+        if key not in self.staging:
+            self.staging[key] = torch.zeros((info.rowsNum * info.pitchBytes + 3) // 4 * 4, dtype=torch.uint8, device=self.stream.device)
+        self.ctx.copy(rtype, index, self.staging[key].data_ptr(), info.pitchBytes, False, self.stream.cuda_stream)
+        return self.tensor(self.staging[key])
+
+    @staticmethod
+    def hex(digests):
+        return {k: "%x.%x.%x" % tuple(int(x) & (2 ** 64 - 1) for x in v.cpu().tolist()) for k, v in digests.items()}
+
+
 def worker(args):
     import torch
     if not torch.cuda.is_available():
@@ -52,27 +82,7 @@ def worker(args):
     gpu = harness.GpuDenoiser(den, W, H)
     ctx, inst = gpu.ctx, gpu.instance
     pipelines = inst.get_instance_desc()["pipelines"]
-    weights = {}
-
-    def digest(buf):
-        v = buf.reshape(-1).view(torch.int32).to(torch.int64)
-        if v.numel() not in weights:
-            i = torch.arange(v.numel(), device=dev, dtype=torch.int64)
-            weights[v.numel()] = ((i % 8191) + 1, (i % 65521) + 1)
-        w1, w2 = weights[v.numel()]
-        return torch.stack([v.sum(), (v * w1).sum(), (v * w2).sum()])
-
-    staging = {}
-
-    def texture_digest(rtype, index):
-        # the texel bytes of the rows the context holds, copied into a buffer of the texture's pitch (padding stays zero)
-        info = ctx.get_texture(rtype, index)
-        key = (int(rtype), index)
-        if key not in staging:
-            staging[key] = torch.zeros((info.rowsNum * info.pitchBytes + 3) // 4 * 4, dtype=torch.uint8, device=dev)
-        ctx.copy(rtype, index, staging[key].data_ptr(), info.pitchBytes, False, stream.cuda_stream)
-        return digest(staging[key])
-
+    dg = Digests(ctx, stream)
     sampler = ClockSampler(0)
     ctx.set_timing(True)
     per_pass, frame_digests, frame_ms = {}, [], []
@@ -98,12 +108,12 @@ def worker(args):
             if name == "Temporal accumulation" and not args.no_digest:
                 for dt, rt, idx in dispatches[j].resources:
                     if dt == nrd.DescriptorType.STORAGE_TEXTURE:
-                        digests["TA:%s[%d]" % (rt.name, idx)] = texture_digest(rt, idx)
+                        digests["TA:%s[%d]" % (rt.name, idx)] = dg.texture(rt, idx)
         for name, t in sorted(gpu.outputs().items()):
             if not args.no_digest:
-                digests[name] = digest(t.contiguous().view(torch.uint8))
+                digests[name] = dg.tensor(t)
         kernel_ms, _ = ctx.get_timing()  # synchronises
-        frame_digests.append({k: "%x.%x.%x" % tuple(int(x) & (2 ** 64 - 1) for x in v.cpu().tolist()) for k, v in digests.items()})
+        frame_digests.append(Digests.hex(digests))
         if len(kernel_ms) != len(names):
             raise RuntimeError("%d timed dispatches for %d dispatch names" % (len(kernel_ms), len(names)))
         if i >= args.warmup:
@@ -181,6 +191,8 @@ def driver(args):
         tas = [r["median_ms"]["Temporal accumulation"] for r in results[name]]
         summary[name] = {"ta_ms_per_round": tas, "ta_ms_median": statistics.median(tas), "ta_spread": (max(tas) - min(tas)) / statistics.median(tas),
                          "per_pass_ms_median": {k: statistics.median([r["median_ms"][k] for r in results[name]]) for k in results[name][0]["median_ms"]},
+                         "per_pass_spread": {k: (max(v) - min(v)) / statistics.median(v) for k in results[name][0]["median_ms"]
+                                             for v in [[r["median_ms"][k] for r in results[name]]]},
                          "sm_mhz": [r["clocks"]["sm_mhz"] for r in results[name]], "digest_mismatches": None if args.no_digest else len(mismatches[name])}
         if args.bench_steps:
             v = benches[name]
