@@ -7,8 +7,6 @@
 #include "../constants.h"
 #include "launch.h"
 
-#include <cstring>
-
 namespace nrdb200
 {
 namespace
@@ -93,20 +91,19 @@ __global__ void __launch_bounds__(256) ReferenceCopyKernel(const __grid_constant
 }
 } // namespace
 
-cudaError_t LaunchAux(const PassLaunch& p, const char* shader)
+cudaError_t LaunchAux(const PassLaunch& p)
 {
     const int rows = p.rowEnd - p.rowBegin;
-    if (rows <= 0) return cudaSuccess;
     const dim3 block(32, 8);
-    const bool reblur = !strncmp(shader, "REBLUR_", 7), relax = !strncmp(shader, "RELAX_", 6);
-    if ((reblur || relax) && strstr(shader, "_SplitScreen.cs"))
+    const Family family = p.kind.family;
+    Bindings b(p);
+    if (family == Family::REBLUR || family == Family::RELAX) // split screen
     {
         SplitArgs a{};
-        const char* s = shader + (reblur ? 7 : 6);
-        a.hasDiff = !strncmp(s, "Diffuse", 7) ? 1 : 0;
-        a.hasSpec = (!strncmp(s, "Specular_", 9) || !strncmp(s, "DiffuseSpecular_", 16)) ? 1 : 0;
+        a.hasDiff = (p.kind.signals & SIGNAL_DIFFUSE) ? 1 : 0;
+        a.hasSpec = (p.kind.signals & SIGNAL_SPECULAR) ? 1 : 0;
         unsigned diffCheckerboard, specCheckerboard;
-        if (reblur)
+        if (family == Family::REBLUR)
         {
             const ReblurConstants& c = *(const ReblurConstants*)p.constants;
             a.rectSizeInvX = c.gRectSizeInv[0]; a.splitScreen = c.gSplitScreen; a.viewZScale = c.gViewZScale; a.denoisingRange = c.gDenoisingRange;
@@ -122,39 +119,38 @@ cudaError_t LaunchAux(const PassLaunch& p, const char* shader)
         }
         a.diffShift = diffCheckerboard != 2 ? 1 : 0;
         a.specShift = specCheckerboard != 2 ? 1 : 0;
-        int k = 0;
-        a.z = p.tex[k++];
-        if (a.hasDiff) a.inDiff = p.tex[k++];
-        if (a.hasSpec) a.inSpec = p.tex[k++];
-        if (a.hasDiff) a.outDiff = p.tex[k++];
-        if (a.hasSpec) a.outSpec = p.tex[k++];
+        a.z = b.Next();
+        a.inDiff = b.Next(a.hasDiff);
+        a.inSpec = b.Next(a.hasSpec);
+        a.outDiff = b.Next(a.hasDiff);
+        a.outSpec = b.Next(a.hasSpec);
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         NRD_B200_LAUNCH(p, dim3((a.rectW + 31) / 32, (rows + 7) / 8), block, a, RadianceSplitScreenKernel);
         return cudaGetLastError();
     }
-    if (!strncmp(shader, "SIGMA_", 6) && strstr(shader, "_SplitScreen.cs"))
+    if (family == Family::SIGMA) // split screen
     {
         const SigmaConstants& c = *(const SigmaConstants*)p.constants;
         SigmaSplitArgs a{};
-        a.translucent = !strncmp(shader, "SIGMA_ShadowTranslucency_", 25) ? 1 : 0;
+        a.translucent = p.kind.translucent ? 1 : 0;
         a.rectSizeInvX = c.gRectSizeInv[0]; a.splitScreen = c.gSplitScreen; a.viewZScale = c.gViewZScale; a.denoisingRange = c.gDenoisingRange;
         a.rectW = c.gRectSizeMinusOne[0] + 1; a.rectH = c.gRectSizeMinusOne[1] + 1;
-        int k = 0;
-        a.z = p.tex[k++]; a.penumbra = p.tex[k++];
-        if (a.translucent) a.translucency = p.tex[k++];
-        a.out = p.tex[k++];
+        a.z = b.Next(); a.penumbra = b.Next(); a.translucency = b.Next(a.translucent); a.out = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         NRD_B200_LAUNCH(p, dim3((a.rectW + 31) / 32, (rows + 7) / 8), block, a, SigmaSplitScreenKernel);
         return cudaGetLastError();
     }
-    if (!strcmp(shader, "REFERENCE_TemporalAccumulation.cs") || !strcmp(shader, "REFERENCE_Copy.cs"))
+    if (family == Family::REFERENCE && (p.kind.pass == Pass::TemporalAccumulation || p.kind.pass == Pass::Copy))
     {
         ReferenceArgs a{};
-        a.in = p.tex[0]; a.out = p.tex[1];
+        a.in = b.Next(); a.out = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.gridW = p.gridW * 16; a.gridH = p.gridH * 16;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         const int w = p.preloadOnly ? 32 : a.out.w;
-        if (!strcmp(shader, "REFERENCE_Copy.cs"))
+        if (p.kind.pass == Pass::Copy)
         {
             const ReferenceCopyConstants& c = *(const ReferenceCopyConstants*)p.constants;
             a.rectSizeInvX = c.gRectSizeInv[0]; a.splitScreen = c.gSplitScreen;

@@ -38,6 +38,25 @@
 namespace nrdb200
 {
 using namespace nrdb200_abi;
+
+// Host side: reads the bindings of a dispatch in the order its recipe binds them (recipes_*.cpp).  Next(false) is a binding the
+// pass does not have (the other signal of a one-signal denoiser): a null surface, and the next binding stays next.  A launcher
+// checks Complete() before it launches: a dispatch that binds more or fewer textures than the pass reads is refused.  Preload
+// launches bind nothing.
+struct Bindings
+{
+    const PassLaunch& p;
+    uint32_t read = 0;
+    explicit Bindings(const PassLaunch& launch) : p(launch) {}
+    Surf Next(bool present = true)
+    {
+        if (!present) return Surf{};
+        const uint32_t i = read++;
+        return i < p.texNum ? p.tex[i] : Surf{};
+    }
+    bool Complete() const { return p.preloadOnly || read == p.texNum; }
+};
+
 // ---------------------------------------------------------------------------------------------
 // Surfaces (surf.h)
 // ---------------------------------------------------------------------------------------------

@@ -1,0 +1,47 @@
+// The one launch entry point of each build of the kernels (launch.h): pass kind -> family launcher.
+#include "launch.h"
+
+namespace nrdb200
+{
+cudaError_t LaunchPass(const PassLaunch& p)
+{
+    if (p.rowEnd <= p.rowBegin) return cudaSuccess; // a rank without rows still takes part in the barriers
+    if (p.kind.pass == Pass::SplitScreen || p.kind.family == Family::REFERENCE) return LaunchAux(p);
+    switch (p.kind.family)
+    {
+        case Family::SIGMA: return LaunchSigma(p);
+        case Family::RELAX: return LaunchRelax(p);
+        case Family::REBLUR:
+            if (p.kind.pass == Pass::ClassifyTiles) return LaunchReblurClassifyTiles(p);
+            // every later pass of the frame reads the decoded guide and the roughness table; the executor provides both
+            if (!p.preloadOnly && (p.guideMode != 2 || !p.roughnessLut)) return cudaErrorInvalidValue;
+            switch (p.kind.pass)
+            {
+                case Pass::HitDistReconstruction:
+                case Pass::HitDistReconstruction_5x5: return LaunchReblurHitDistReconstruction(p);
+                case Pass::PrePass: return LaunchReblurPrePass(p);
+                case Pass::TemporalAccumulation: return LaunchReblurTemporalAccumulation(p);
+                case Pass::HistoryFix: return LaunchReblurHistoryFix(p);
+                case Pass::Blur: return LaunchReblurBlur(p);
+                case Pass::PostBlur:
+                case Pass::PostBlur_NoTemporalStabilization: return LaunchReblurPostBlur(p);
+                case Pass::TemporalStabilization: return LaunchReblurTemporalStabilization(p);
+                default: return cudaErrorNotSupported;
+            }
+        default: return cudaErrorNotSupported; // CLEAR: the executor clears itself
+    }
+}
+
+#if !defined(NRD_B200_NO_STRIPS)
+cudaError_t SetPeerTables(int slot, const PeerTable* table)
+{
+    cudaError_t e = SetPeerTableReblurSpatial(slot, table);
+    if (e == cudaSuccess) e = SetPeerTableReblurHitDist(slot, table);
+    if (e == cudaSuccess) e = SetPeerTableReblurTemporal(slot, table);
+    if (e == cudaSuccess) e = SetPeerTableSigma(slot, table);
+    if (e == cudaSuccess) e = SetPeerTableRelax(slot, table);
+    if (e == cudaSuccess) e = SetPeerTableAux(slot, table);
+    return e;
+}
+#endif
+} // namespace nrdb200

@@ -1,36 +1,37 @@
-// Host-visible launchers of the sm_90a kernels (one per reference pass).  `signal`: 0 = diffuse, 1 = specular, 2 = both.
-// Every kernel translation unit is compiled twice (common.cuh): NS = nrdb200 is the strip (multi-GPU) build,
-// NS = nrdb200_single the one-GPU build.
+// Host-visible launchers of the sm_90a kernels.  Every kernel translation unit is compiled twice (common.cuh): NS = nrdb200 is
+// the strip (multi-GPU) build, NS = nrdb200_single the one-GPU build.  The executor calls LaunchPass of one build; LaunchPass
+// (dispatch.cu) picks the family launcher from PassLaunch::kind, and the family launcher picks the kernel.
 #pragma once
 #include "common.cuh"
 
-#define NRD_B200_DECLARE_LAUNCHERS(NS)                                                                          \
-    namespace NS                                                                                                \
-    {                                                                                                           \
-    cudaError_t LaunchReblurClassifyTiles(const nrdb200_abi::PassLaunch& p);                                    \
-    cudaError_t LaunchReblurHitDistReconstruction(const nrdb200_abi::PassLaunch& p, int signal, bool is5x5);   \
-    cudaError_t LaunchReblurPrePass(const nrdb200_abi::PassLaunch& p, int signal);                              \
-    cudaError_t LaunchReblurTemporalAccumulation(const nrdb200_abi::PassLaunch& p, int signal);                 \
-    cudaError_t LaunchReblurHistoryFix(const nrdb200_abi::PassLaunch& p, int signal);                           \
-    cudaError_t LaunchReblurBlur(const nrdb200_abi::PassLaunch& p, int signal);                                 \
-    cudaError_t LaunchReblurPostBlur(const nrdb200_abi::PassLaunch& p, int signal, bool noTemporalStabilization); \
-    cudaError_t LaunchReblurTemporalStabilization(const nrdb200_abi::PassLaunch& p, int signal);                \
-    cudaError_t LaunchSigma(const nrdb200_abi::PassLaunch& p, const char* shaderName);                          \
-    cudaError_t LaunchRelax(const nrdb200_abi::PassLaunch& p, const char* shaderName);                          \
-    cudaError_t LaunchAux(const nrdb200_abi::PassLaunch& p, const char* shaderName);                            \
-    }
-
-NRD_B200_DECLARE_LAUNCHERS(nrdb200)
-
-#if !defined(NRD_B200_NO_STRIPS)
 namespace nrdb200
 {
+cudaError_t LaunchReblurClassifyTiles(const PassLaunch& p);
+cudaError_t LaunchReblurHitDistReconstruction(const PassLaunch& p);
+cudaError_t LaunchReblurPrePass(const PassLaunch& p);
+cudaError_t LaunchReblurTemporalAccumulation(const PassLaunch& p);
+cudaError_t LaunchReblurHistoryFix(const PassLaunch& p);
+cudaError_t LaunchReblurBlur(const PassLaunch& p);
+cudaError_t LaunchReblurPostBlur(const PassLaunch& p);
+cudaError_t LaunchReblurTemporalStabilization(const PassLaunch& p);
+cudaError_t LaunchSigma(const PassLaunch& p);
+cudaError_t LaunchRelax(const PassLaunch& p);
+cudaError_t LaunchAux(const PassLaunch& p); // split-screen passes, REFERENCE denoiser
+cudaError_t LaunchPass(const PassLaunch& p); // cudaErrorNotSupported: the pass has no kernel
+
+#if !defined(NRD_B200_NO_STRIPS)
 // peer address table of one context slot, replicated into the constant memory of every kernel translation unit
-cudaError_t SetPeerTableReblurSpatial(int slot, const nrdb200_abi::PeerTable* table);
-cudaError_t SetPeerTableReblurHitDist(int slot, const nrdb200_abi::PeerTable* table);
-cudaError_t SetPeerTableReblurTemporal(int slot, const nrdb200_abi::PeerTable* table);
-cudaError_t SetPeerTableSigma(int slot, const nrdb200_abi::PeerTable* table);
-cudaError_t SetPeerTableRelax(int slot, const nrdb200_abi::PeerTable* table);
-cudaError_t SetPeerTableAux(int slot, const nrdb200_abi::PeerTable* table);
-} // namespace nrdb200
+cudaError_t SetPeerTableReblurSpatial(int slot, const PeerTable* table);
+cudaError_t SetPeerTableReblurHitDist(int slot, const PeerTable* table);
+cudaError_t SetPeerTableReblurTemporal(int slot, const PeerTable* table);
+cudaError_t SetPeerTableSigma(int slot, const PeerTable* table);
+cudaError_t SetPeerTableRelax(int slot, const PeerTable* table);
+cudaError_t SetPeerTableAux(int slot, const PeerTable* table);
+cudaError_t SetPeerTables(int slot, const PeerTable* table); // all of the above
 #endif
+} // namespace nrdb200
+
+namespace nrdb200_single
+{
+cudaError_t LaunchPass(const nrdb200_abi::PassLaunch& p);
+}

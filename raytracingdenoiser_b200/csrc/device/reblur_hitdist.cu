@@ -142,19 +142,19 @@ __global__ void __launch_bounds__(kHdTileW* kHdTileH) ReblurHitDistReconstructio
 
 template <bool DIFF, bool SPEC, int BORDER> static cudaError_t LaunchHitDist(const PassLaunch& p)
 {
-    if (!p.preloadOnly && (p.guideMode != 2 || !p.roughnessLut)) return cudaErrorInvalidValue;
     HitDistArgs a;
     a.c = *(const ReblurConstants*)p.constants;
-    int k = 0;
-    a.tiles = p.tex[k++];
-    a.nr = p.tex[k++];
-    k++; // IN_VIEWZ: the guide surface carries it
-    if (DIFF) a.inDiff = p.tex[k++];
-    if (SPEC) a.inSpec = p.tex[k++];
-    if (DIFF) a.outDiff = p.tex[k++];
-    if (SPEC) a.outSpec = p.tex[k++];
+    Bindings b(p);
+    a.tiles = b.Next();
+    a.nr = b.Next();
+    b.Next(); // IN_VIEWZ: the guide surface carries it
+    a.inDiff = b.Next(DIFF);
+    a.inSpec = b.Next(SPEC);
+    a.outDiff = b.Next(DIFF);
+    a.outSpec = b.Next(SPEC);
+    if (!b.Complete()) return cudaErrorInvalidValue;
     a.guide = p.guide;
-    a.perf = p.performanceMode ? 1 : 0;
+    a.perf = p.kind.perf ? 1 : 0;
     a.lut = (const float4*)p.roughnessLut;
     a.rowBegin = p.rowBegin;
     a.rowEnd = p.rowEnd;
@@ -172,10 +172,11 @@ template <bool DIFF, bool SPEC, int BORDER> static cudaError_t LaunchHitDist(con
     return cudaGetLastError();
 }
 
-cudaError_t LaunchReblurHitDistReconstruction(const PassLaunch& p, int signal, bool is5x5)
+cudaError_t LaunchReblurHitDistReconstruction(const PassLaunch& p)
 {
-    if (signal == 0) return is5x5 ? LaunchHitDist<true, false, 2>(p) : LaunchHitDist<true, false, 1>(p);
-    if (signal == 1) return is5x5 ? LaunchHitDist<false, true, 2>(p) : LaunchHitDist<false, true, 1>(p);
+    const bool is5x5 = p.kind.pass == Pass::HitDistReconstruction_5x5;
+    if (p.kind.signals == SIGNAL_DIFFUSE) return is5x5 ? LaunchHitDist<true, false, 2>(p) : LaunchHitDist<true, false, 1>(p);
+    if (p.kind.signals == SIGNAL_SPECULAR) return is5x5 ? LaunchHitDist<false, true, 2>(p) : LaunchHitDist<false, true, 1>(p);
     return is5x5 ? LaunchHitDist<true, true, 2>(p) : LaunchHitDist<true, true, 1>(p);
 }
 

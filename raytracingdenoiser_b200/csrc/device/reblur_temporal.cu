@@ -1254,28 +1254,27 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchTa(const PassLaunch& p)
     a.c = *(const ReblurConstants*)p.constants;
     a.guide = p.guide;
     a.lut = (const float4*)p.roughnessLut;
-    if (!p.preloadOnly && (p.guideMode != 2 || !p.roughnessLut)) return cudaErrorInvalidValue; // the executor always provides both
-    int k = 0;
-    a.tiles = p.tex[k++]; a.nr = p.tex[k++]; a.z = p.tex[k++]; a.mv = p.tex[k++];
-    a.prevZ = p.tex[k++]; a.prevNr = p.tex[k++]; a.prevInternal = p.tex[k++];
-    a.mix = p.tex[k++];                      // gIn_DisocclusionThresholdMix (bound to IN_VIEWZ when absent, never read then)
-    if (DIFF) a.diffConfidence = p.tex[k++]; // gIn_DiffConfidence
-    if (SPEC) a.specConfidence = p.tex[k++]; // gIn_SpecConfidence
-    if (DIFF) a.inDiff = p.tex[k++];
-    if (SPEC) a.inSpec = p.tex[k++];
-    if (DIFF && SPEC) { a.histDiff = p.tex[k++]; a.histSpec = p.tex[k++]; a.histDiffFast = p.tex[k++]; a.histSpecFast = p.tex[k++]; }
-    else if (DIFF) { a.histDiff = p.tex[k++]; a.histDiffFast = p.tex[k++]; }
-    else { a.histSpec = p.tex[k++]; a.histSpecFast = p.tex[k++]; }
-    if (SPEC) { a.prevHitDist = p.tex[k++]; a.inHitDist = p.tex[k++]; }
-    if (DIFF) a.outDiff = p.tex[k++];
-    if (SPEC) a.outSpec = p.tex[k++];
-    if (DIFF) a.outDiffFast = p.tex[k++];
-    if (SPEC) { a.outSpecFast = p.tex[k++]; a.outHitDist = p.tex[k++]; }
-    a.outData1 = p.tex[k++];
-    a.outData2 = p.tex[k++];
+    Bindings b(p);
+    a.tiles = b.Next(); a.nr = b.Next(); a.z = b.Next(); a.mv = b.Next();
+    a.prevZ = b.Next(); a.prevNr = b.Next(); a.prevInternal = b.Next();
+    a.mix = b.Next();                      // gIn_DisocclusionThresholdMix (bound to IN_VIEWZ when absent, never read then)
+    a.diffConfidence = b.Next(DIFF);       // gIn_DiffConfidence
+    a.specConfidence = b.Next(SPEC);       // gIn_SpecConfidence
+    a.inDiff = b.Next(DIFF);
+    a.inSpec = b.Next(SPEC);
+    if (DIFF && SPEC) { a.histDiff = b.Next(); a.histSpec = b.Next(); a.histDiffFast = b.Next(); a.histSpecFast = b.Next(); }
+    else { a.histDiff = b.Next(DIFF); a.histDiffFast = b.Next(DIFF); a.histSpec = b.Next(SPEC); a.histSpecFast = b.Next(SPEC); }
+    a.prevHitDist = b.Next(SPEC); a.inHitDist = b.Next(SPEC);
+    a.outDiff = b.Next(DIFF);
+    a.outSpec = b.Next(SPEC);
+    a.outDiffFast = b.Next(DIFF);
+    a.outSpecFast = b.Next(SPEC); a.outHitDist = b.Next(SPEC);
+    a.outData1 = b.Next();
+    a.outData2 = b.Next();
+    if (!b.Complete()) return cudaErrorInvalidValue;
     a.rowBegin = p.rowBegin;
     a.rowEnd = p.rowEnd;
-    a.perf = p.performanceMode ? 1 : 0;
+    a.perf = p.kind.perf ? 1 : 0;
     const int W = (int)a.c.gRectSize[0];
     dim3 grid((W + 31) / 32, (p.rowEnd - p.rowBegin + 3) / 4), block(32, 4);
     // the switches ReblurTemporalAccumulationKernel<DIFF, SPEC> compiles as constants
@@ -1286,10 +1285,10 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchTa(const PassLaunch& p)
     if (isDefault || p.preloadOnly) NRD_B200_LAUNCH(p, grid, block, a, ReblurTemporalAccumulationKernel<DIFF, SPEC>);
     return cudaGetLastError();
 }
-cudaError_t LaunchReblurTemporalAccumulation(const PassLaunch& p, int signal)
+cudaError_t LaunchReblurTemporalAccumulation(const PassLaunch& p)
 {
-    if (signal == 0) return LaunchTa<true, false>(p);
-    if (signal == 1) return LaunchTa<false, true>(p);
+    if (p.kind.signals == SIGNAL_DIFFUSE) return LaunchTa<true, false>(p);
+    if (p.kind.signals == SIGNAL_SPECULAR) return LaunchTa<false, true>(p);
     return LaunchTa<true, true>(p);
 }
 
@@ -1299,20 +1298,20 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchHf(const PassLaunch& p)
     a.c = *(const ReblurConstants*)p.constants;
     a.guide = p.guide;
     a.lut = (const float4*)p.roughnessLut;
-    if (!p.preloadOnly && (p.guideMode != 2 || !p.roughnessLut)) return cudaErrorInvalidValue; // the executor always provides both
-    int k = 0;
-    a.tiles = p.tex[k++]; a.nr = p.tex[k++]; a.data1 = p.tex[k++]; a.z = p.tex[k++];
-    if (DIFF) a.inDiff = p.tex[k++];
-    if (SPEC) a.inSpec = p.tex[k++];
-    if (DIFF) a.inDiffFast = p.tex[k++];
-    if (SPEC) a.inSpecFast = p.tex[k++];
-    if (DIFF) a.outDiff = p.tex[k++];
-    if (SPEC) a.outSpec = p.tex[k++];
-    if (DIFF) a.outDiffFast = p.tex[k++];
-    if (SPEC) a.outSpecFast = p.tex[k++];
+    Bindings b(p);
+    a.tiles = b.Next(); a.nr = b.Next(); a.data1 = b.Next(); a.z = b.Next();
+    a.inDiff = b.Next(DIFF);
+    a.inSpec = b.Next(SPEC);
+    a.inDiffFast = b.Next(DIFF);
+    a.inSpecFast = b.Next(SPEC);
+    a.outDiff = b.Next(DIFF);
+    a.outSpec = b.Next(SPEC);
+    a.outDiffFast = b.Next(DIFF);
+    a.outSpecFast = b.Next(SPEC);
+    if (!b.Complete()) return cudaErrorInvalidValue;
     a.rowBegin = p.rowBegin;
     a.rowEnd = p.rowEnd;
-    a.perf = p.performanceMode ? 1 : 0;
+    a.perf = p.kind.perf ? 1 : 0;
     const int W = (int)a.c.gRectSize[0];
     dim3 grid((W + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8), block(32, 8);
     if (p.preloadOnly)
@@ -1329,10 +1328,10 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchHf(const PassLaunch& p)
     ReblurHistoryFixKernel<DIFF, SPEC><<<grid, block, 0, p.stream>>>(a, diffMap, specMap);
     return cudaGetLastError();
 }
-cudaError_t LaunchReblurHistoryFix(const PassLaunch& p, int signal)
+cudaError_t LaunchReblurHistoryFix(const PassLaunch& p)
 {
-    if (signal == 0) return LaunchHf<true, false>(p);
-    if (signal == 1) return LaunchHf<false, true>(p);
+    if (p.kind.signals == SIGNAL_DIFFUSE) return LaunchHf<true, false>(p);
+    if (p.kind.signals == SIGNAL_SPECULAR) return LaunchHf<false, true>(p);
     return LaunchHf<true, true>(p);
 }
 
@@ -1342,24 +1341,24 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchTs(const PassLaunch& p)
     a.c = *(const ReblurConstants*)p.constants;
     a.guide = p.guide;
     a.lut = (const float4*)p.roughnessLut;
-    if (!p.preloadOnly && (p.guideMode != 2 || !p.roughnessLut)) return cudaErrorInvalidValue; // the executor always provides both
-    int k = 0;
-    a.tiles = p.tex[k++]; a.nr = p.tex[k++];
-    if (SPEC) a.baseColorMetalness = p.tex[k++]; // gIn_BaseColor_Metalness (bound to IN_VIEWZ when absent, never read then)
-    a.z = p.tex[k++]; a.data1 = p.tex[k++]; a.data2 = p.tex[k++];
-    if (DIFF) a.inDiff = p.tex[k++];
-    if (SPEC) a.inSpec = p.tex[k++];
-    if (DIFF) a.histDiffStab = p.tex[k++];
-    if (SPEC) { a.histSpecStab = p.tex[k++]; a.hitDist = p.tex[k++]; }
-    a.mv = p.tex[k++];
-    a.outInternal = p.tex[k++];
-    if (DIFF) a.outDiff = p.tex[k++];
-    if (SPEC) a.outSpec = p.tex[k++];
-    if (DIFF) a.outDiffStab = p.tex[k++];
-    if (SPEC) a.outSpecStab = p.tex[k++];
+    Bindings b(p);
+    a.tiles = b.Next(); a.nr = b.Next();
+    a.baseColorMetalness = b.Next(SPEC); // gIn_BaseColor_Metalness (bound to IN_VIEWZ when absent, never read then)
+    a.z = b.Next(); a.data1 = b.Next(); a.data2 = b.Next();
+    a.inDiff = b.Next(DIFF);
+    a.inSpec = b.Next(SPEC);
+    a.histDiffStab = b.Next(DIFF);
+    a.histSpecStab = b.Next(SPEC); a.hitDist = b.Next(SPEC);
+    a.mv = b.Next();
+    a.outInternal = b.Next();
+    a.outDiff = b.Next(DIFF);
+    a.outSpec = b.Next(SPEC);
+    a.outDiffStab = b.Next(DIFF);
+    a.outSpecStab = b.Next(SPEC);
+    if (!b.Complete()) return cudaErrorInvalidValue;
     a.rowBegin = p.rowBegin;
     a.rowEnd = p.rowEnd;
-    a.perf = p.performanceMode ? 1 : 0;
+    a.perf = p.kind.perf ? 1 : 0;
     const int W = (int)a.c.gRectSize[0];
     dim3 grid((W + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8), block(32, 8);
     if (p.preloadOnly)
@@ -1377,10 +1376,10 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchTs(const PassLaunch& p)
     ReblurTemporalStabilizationKernel<DIFF, SPEC><<<grid, block, 0, p.stream>>>(a, diffMap, specMap);
     return cudaGetLastError();
 }
-cudaError_t LaunchReblurTemporalStabilization(const PassLaunch& p, int signal)
+cudaError_t LaunchReblurTemporalStabilization(const PassLaunch& p)
 {
-    if (signal == 0) return LaunchTs<true, false>(p);
-    if (signal == 1) return LaunchTs<false, true>(p);
+    if (p.kind.signals == SIGNAL_DIFFUSE) return LaunchTs<true, false>(p);
+    if (p.kind.signals == SIGNAL_SPECULAR) return LaunchTs<false, true>(p);
     return LaunchTs<true, true>(p);
 }
 

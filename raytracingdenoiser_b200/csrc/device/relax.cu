@@ -1567,122 +1567,113 @@ template <bool DIFF, bool SPEC> __global__ void __launch_bounds__(256) RelaxAtro
 
 // ---------------------------------------------------------------------------------------------
 // RELAX_Diffuse_* / RELAX_Specular_* are the two-signal passes without the other signal's bindings (Source/Denoisers/Relax_Diffuse.hpp,
-// Relax_Specular.hpp): a one-signal dispatch is expanded to the two-signal binding layout below (c = common, s = specular only,
-// d = diffuse only; absent bindings stay null surfaces, the kernels are compiled without every access to them).
-struct RelaxPassLayout
-{
-    const char* pass;
-    const char* layout;
-};
-static const RelaxPassLayout kRelaxLayouts[] = {
-    {"HitDistReconstruction.cs", "csdccsd"},
-    {"HitDistReconstruction_5x5.cs", "csdccsd"},
-    {"PrePass.cs", "csdccsd"},
-    {"TemporalAccumulation.cs", "csdcccsdsdccsccsdcsdsdscs"},
-    {"HistoryFix.cs", "csdcccsd"},
-    {"HistoryClamping.cs", "ccsdsdsdcsdsdc"},
-    {"Copy.cs", "sdsd"},
-    {"AntiFirefly.cs", "csdccsd"},
-    {"AtrousSmem.cs", "csdcsccsdsdccc"},
-    {"Atrous.cs", "csdcsccsdsd"},
-};
-
-template <bool DIFF, bool SPEC> static cudaError_t LaunchRelaxSignals(const PassLaunch& p, const char* shader, const RC& c)
+// Relax_Specular.hpp): the bindings of the absent signal are null surfaces, the kernels are compiled without every access to them.
+template <bool DIFF, bool SPEC> static cudaError_t LaunchRelaxSignals(const PassLaunch& p, const RC& c)
 {
     const int W = c.gRectSize[0];
     const int rows = p.rowEnd - p.rowBegin;
     const dim3 block(32, 8), grid((W + 31) / 32, (rows + 7) / 8);
-    if (!strcmp(shader, "HitDistReconstruction.cs") || !strcmp(shader, "HitDistReconstruction_5x5.cs"))
+    Bindings b(p);
+    if (p.kind.pass == Pass::HitDistReconstruction || p.kind.pass == Pass::HitDistReconstruction_5x5)
     {
         RxHitDistArgs a;
         a.c = c;
         a.guide = p.guide;
-        a.tiles = p.tex[0]; a.spec = p.tex[1]; a.diff = p.tex[2]; a.nr = p.tex[3]; a.z = p.tex[4]; a.outSpec = p.tex[5]; a.outDiff = p.tex[6];
+        a.tiles = b.Next(); a.spec = b.Next(SPEC); a.diff = b.Next(DIFF); a.nr = b.Next(); a.z = b.Next(); a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF);
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
-        if (!strcmp(shader, "HitDistReconstruction.cs")) NRD_B200_LAUNCH(p, grid, block, a, RelaxHitDistReconstructionKernel<DIFF, SPEC, 1>);
+        if (p.kind.pass == Pass::HitDistReconstruction) NRD_B200_LAUNCH(p, grid, block, a, RelaxHitDistReconstructionKernel<DIFF, SPEC, 1>);
         else NRD_B200_LAUNCH(p, grid, block, a, RelaxHitDistReconstructionKernel<DIFF, SPEC, 2>);
     }
-    else if (!strcmp(shader, "PrePass.cs"))
+    else if (p.kind.pass == Pass::PrePass)
     {
         RxPrePassArgs a;
         a.c = c;
         a.guide = p.guide;
-        a.tiles = p.tex[0]; a.spec = p.tex[1]; a.diff = p.tex[2]; a.nr = p.tex[3]; a.z = p.tex[4]; a.outSpec = p.tex[5]; a.outDiff = p.tex[6];
+        a.tiles = b.Next(); a.spec = b.Next(SPEC); a.diff = b.Next(DIFF); a.nr = b.Next(); a.z = b.Next(); a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF);
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         const bool checkerboard = (DIFF && c.gDiffCheckerboard != 2u) || (SPEC && c.gSpecCheckerboard != 2u);
         if (checkerboard || p.preloadOnly) NRD_B200_LAUNCH(p, grid, block, a, RelaxPrePassKernel<DIFF, SPEC, true>);
         if (!checkerboard || p.preloadOnly) NRD_B200_LAUNCH(p, grid, block, a, RelaxPrePassKernel<DIFF, SPEC>);
     }
-    else if (!strcmp(shader, "TemporalAccumulation.cs"))
+    else if (p.kind.pass == Pass::TemporalAccumulation)
     {
         RxTaArgs a;
         a.c = c;
         a.guide = p.guide;
-        a.tiles = p.tex[0]; a.spec = p.tex[1]; a.diff = p.tex[2]; a.mv = p.tex[3]; a.nr = p.tex[4]; a.z = p.tex[5];
-        a.histSpecFast = p.tex[6]; a.histDiffFast = p.tex[7]; a.histSpec = p.tex[8]; a.histDiff = p.tex[9];
-        a.prevNr = p.tex[10]; a.prevZ = p.tex[11]; a.prevHitDist = p.tex[12]; a.prevLength = p.tex[13]; a.prevMaterial = p.tex[14];
-        a.specConfidence = p.tex[15]; a.diffConfidence = p.tex[16]; a.mix = p.tex[17]; // bound to IN_VIEWZ when absent, never read then
-        a.outSpec = p.tex[18]; a.outDiff = p.tex[19]; a.outSpecFast = p.tex[20]; a.outDiffFast = p.tex[21]; a.outHitDist = p.tex[22]; a.outLength = p.tex[23];
-        a.outConfidence = p.tex[24];
+        a.tiles = b.Next(); a.spec = b.Next(SPEC); a.diff = b.Next(DIFF); a.mv = b.Next(); a.nr = b.Next(); a.z = b.Next();
+        a.histSpecFast = b.Next(SPEC); a.histDiffFast = b.Next(DIFF); a.histSpec = b.Next(SPEC); a.histDiff = b.Next(DIFF);
+        a.prevNr = b.Next(); a.prevZ = b.Next(); a.prevHitDist = b.Next(SPEC); a.prevLength = b.Next(); a.prevMaterial = b.Next();
+        a.specConfidence = b.Next(SPEC); a.diffConfidence = b.Next(DIFF); a.mix = b.Next(); // bound to IN_VIEWZ when absent, never read then
+        a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF); a.outSpecFast = b.Next(SPEC); a.outDiffFast = b.Next(DIFF); a.outHitDist = b.Next(SPEC);
+        a.outLength = b.Next(); a.outConfidence = b.Next(SPEC);
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         const bool checkerboard = (DIFF && c.gDiffCheckerboard != 2u) || (SPEC && c.gSpecCheckerboard != 2u);
         if (checkerboard || p.preloadOnly) NRD_B200_LAUNCH(p, dim3((W + 31) / 32, (rows + 3) / 4), dim3(32, 4), a, RelaxTemporalAccumulationKernel<DIFF, SPEC, true>);
         if (!checkerboard || p.preloadOnly) NRD_B200_LAUNCH(p, dim3((W + 31) / 32, (rows + 3) / 4), dim3(32, 4), a, RelaxTemporalAccumulationKernel<DIFF, SPEC>);
     }
-    else if (!strcmp(shader, "HistoryFix.cs"))
+    else if (p.kind.pass == Pass::HistoryFix)
     {
         RxHfArgs a;
         a.c = c;
         a.guide = p.guide;
-        a.tiles = p.tex[0]; a.spec = p.tex[1]; a.diff = p.tex[2]; a.length = p.tex[3]; a.nr = p.tex[4]; a.z = p.tex[5]; a.outSpec = p.tex[6]; a.outDiff = p.tex[7];
+        a.tiles = b.Next(); a.spec = b.Next(SPEC); a.diff = b.Next(DIFF); a.length = b.Next(); a.nr = b.Next(); a.z = b.Next(); a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF);
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         NRD_B200_LAUNCH(p, grid, block, a, RelaxHistoryFixKernel<DIFF, SPEC>);
     }
-    else if (!strcmp(shader, "HistoryClamping.cs"))
+    else if (p.kind.pass == Pass::HistoryClamping)
     {
         RxHcArgs a;
         a.c = c;
-        a.tiles = p.tex[0]; a.z = p.tex[1]; a.specNoisy = p.tex[2]; a.diffNoisy = p.tex[3]; a.spec = p.tex[4]; a.diff = p.tex[5]; a.specFast = p.tex[6]; a.diffFast = p.tex[7];
-        a.length = p.tex[8];
-        a.outSpec = p.tex[9]; a.outDiff = p.tex[10]; a.outSpecFast = p.tex[11]; a.outDiffFast = p.tex[12]; a.outLength = p.tex[13];
+        a.tiles = b.Next(); a.z = b.Next(); a.specNoisy = b.Next(SPEC); a.diffNoisy = b.Next(DIFF); a.spec = b.Next(SPEC); a.diff = b.Next(DIFF);
+        a.specFast = b.Next(SPEC); a.diffFast = b.Next(DIFF); a.length = b.Next();
+        a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF); a.outSpecFast = b.Next(SPEC); a.outDiffFast = b.Next(DIFF); a.outLength = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         NRD_B200_LAUNCH(p, grid, block, a, RelaxHistoryClampingKernel<DIFF, SPEC>);
     }
-    else if (!strcmp(shader, "Copy.cs"))
+    else if (p.kind.pass == Pass::Copy)
     {
         RxCopyArgs a;
-        a.inSpec = p.tex[0]; a.inDiff = p.tex[1]; a.outSpec = p.tex[2]; a.outDiff = p.tex[3];
+        a.inSpec = b.Next(SPEC); a.inDiff = b.Next(DIFF); a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF);
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.gridW = p.gridW * 8; a.gridH = p.gridH * 8;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         NRD_B200_LAUNCH(p, dim3(((SPEC ? a.outSpec.w : a.outDiff.w) + 31) / 32, grid.y), block, a, RelaxCopyKernel<DIFF, SPEC>);
     }
-    else if (!strcmp(shader, "AntiFirefly.cs"))
+    else if (p.kind.pass == Pass::AntiFirefly)
     {
         RxAfArgs a;
         a.c = c;
-        a.tiles = p.tex[0]; a.spec = p.tex[1]; a.diff = p.tex[2]; a.nr = p.tex[3]; a.z = p.tex[4]; a.outSpec = p.tex[5]; a.outDiff = p.tex[6];
+        a.tiles = b.Next(); a.spec = b.Next(SPEC); a.diff = b.Next(DIFF); a.nr = b.Next(); a.z = b.Next(); a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF);
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         NRD_B200_LAUNCH(p, grid, block, a, RelaxAntiFireflyKernel<DIFF, SPEC>);
     }
-    else if (!strcmp(shader, "AtrousSmem.cs") || !strcmp(shader, "Atrous.cs"))
+    else if (p.kind.pass == Pass::AtrousSmem || p.kind.pass == Pass::Atrous)
     {
-        const bool smem = !strcmp(shader, "AtrousSmem.cs");
+        const bool smem = p.kind.pass == Pass::AtrousSmem;
         RxAtrousArgs a;
         a.c = c;
         a.guide = p.guide;
-        a.tiles = p.tex[0]; a.spec = p.tex[1]; a.diff = p.tex[2]; a.length = p.tex[3]; a.confidence = p.tex[4]; a.nr = p.tex[5]; a.z = p.tex[6];
-        a.specConfidence = p.tex[7]; a.diffConfidence = p.tex[8];
-        a.outSpec = p.tex[9]; a.outDiff = p.tex[10];
+        a.tiles = b.Next(); a.spec = b.Next(SPEC); a.diff = b.Next(DIFF); a.length = b.Next(); a.confidence = b.Next(SPEC); a.nr = b.Next(); a.z = b.Next();
+        a.specConfidence = b.Next(SPEC); a.diffConfidence = b.Next(DIFF);
+        a.outSpec = b.Next(SPEC); a.outDiff = b.Next(DIFF);
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         if (smem)
         {
-            a.outNr = p.tex[11]; a.outMaterial = p.tex[12]; a.outZ = p.tex[13];
+            a.outNr = b.Next(); a.outMaterial = b.Next(); a.outZ = b.Next();
+            if (!b.Complete()) return cudaErrorInvalidValue;
             a.gridW = p.gridW * 8; a.gridH = p.gridH * 8;
             const int coverW = min(a.gridW, p.preloadOnly ? 32 : a.outZ.w), coverRows = min(p.rowEnd, a.gridH) - p.rowBegin;
             NRD_B200_LAUNCH(p, dim3((coverW + 31) / 32, (max(coverRows, 1) + 7) / 8), block, a, RelaxAtrousSmemKernel<DIFF, SPEC>);
         }
         else
         {
+            if (!b.Complete()) return cudaErrorInvalidValue;
             a.outNr = a.outMaterial = a.outZ = a.z;
             NRD_B200_LAUNCH(p, grid, block, a, RelaxAtrousKernel<DIFF, SPEC>);
         }
@@ -1692,48 +1683,26 @@ template <bool DIFF, bool SPEC> static cudaError_t LaunchRelaxSignals(const Pass
     return cudaGetLastError();
 }
 
-cudaError_t LaunchRelax(const PassLaunch& p, const char* shader)
+cudaError_t LaunchRelax(const PassLaunch& p)
 {
     RC c;
     memset(&c, 0, sizeof(c));
     memcpy(&c, p.constants, p.constantsSize < sizeof(RC) ? p.constantsSize : sizeof(RC));
-    if (p.rowEnd - p.rowBegin <= 0) return cudaSuccess;
-    if (!strcmp(shader, "RELAX_ClassifyTiles.cs"))
+    if (p.kind.pass == Pass::ClassifyTiles)
     {
         RxTilesArgs a;
+        Bindings b(p);
+        a.z = b.Next(); a.tiles = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.nr = p.guideNr; a.guide = p.guide; a.buildGuide = p.guideMode == 1 ? 1 : 0;
-        a.z = p.tex[0]; a.tiles = p.tex[1];
         a.denoisingRange = c.gDenoisingRange; a.tilesW = p.gridW; a.tilesH = p.gridH;
         int warps = a.tilesW * a.tilesH;
         NRD_B200_LAUNCH(p, (warps * 32 + 255) / 256, 256, a, RelaxClassifyTilesKernel);
         return cudaGetLastError();
     }
-    if (strncmp(shader, "RELAX_", 6) != 0) return cudaErrorNotSupported;
-    const char* pass = shader + 6;
-    bool hasDiff = false, hasSpec = false;
-    if (!strncmp(pass, "DiffuseSpecular_", 16)) { hasDiff = hasSpec = true; pass += 16; }
-    else if (!strncmp(pass, "Diffuse_", 8)) { hasDiff = true; pass += 8; }
-    else if (!strncmp(pass, "Specular_", 9)) { hasSpec = true; pass += 9; }
-    else return cudaErrorNotSupported;
-    const RelaxPassLayout* layout = nullptr;
-    for (const RelaxPassLayout& l : kRelaxLayouts)
-        if (!strcmp(pass, l.pass)) layout = &l;
-    if (!layout) return cudaErrorNotSupported;
-    PassLaunch q = p;
-    for (Surf& t : q.tex) t = Surf{};
-    uint32_t k = 0;
-    for (uint32_t i = 0; layout->layout[i]; i++)
-    {
-        const char kind = layout->layout[i];
-        if (kind == 'c' || (kind == 's' && hasSpec) || (kind == 'd' && hasDiff))
-        {
-            if (k >= p.texNum && !p.preloadOnly) return cudaErrorInvalidValue;
-            q.tex[i] = p.tex[k++];
-        }
-    }
-    if (k != p.texNum && !p.preloadOnly) return cudaErrorInvalidValue;
-    if (hasDiff && hasSpec) return LaunchRelaxSignals<true, true>(q, pass, c);
-    return hasDiff ? LaunchRelaxSignals<true, false>(q, pass, c) : LaunchRelaxSignals<false, true>(q, pass, c);
+    if (p.kind.signals == SIGNAL_DIFFUSE) return LaunchRelaxSignals<true, false>(p, c);
+    if (p.kind.signals == SIGNAL_SPECULAR) return LaunchRelaxSignals<false, true>(p, c);
+    return LaunchRelaxSignals<true, true>(p, c);
 }
 
 #if !defined(NRD_B200_NO_STRIPS)

@@ -504,52 +504,52 @@ __global__ void __launch_bounds__(256) SigmaTemporalStabilizationKernel(const __
 }
 
 // ---------------------------------------------------------------------------------------------
-cudaError_t LaunchSigma(const PassLaunch& p, const char* shader)
+cudaError_t LaunchSigma(const PassLaunch& p)
 {
     const SigmaConstants& c = *(const SigmaConstants*)p.constants;
     const int W = (int)c.gRectSize[0];
-    // "SIGMA_Shadow_<pass>.cs" (SIGMA_TYPE float) / "SIGMA_ShadowTranslucency_<pass>.cs" (float4); SmoothTiles and Copy are shared, Copy
-    // sees which one it serves from the format of the history texture (p.texBytes)
-    const bool translucent = !strncmp(shader, "SIGMA_ShadowTranslucency_", 25);
-    const char* pass = translucent ? shader + 25 : (!strncmp(shader, "SIGMA_Shadow_", 13) ? shader + 13 : shader);
-    if (!strcmp(pass, "ClassifyTiles.cs"))
+    // SIGMA_TYPE float (SIGMA_Shadow_*) or float4 (SIGMA_ShadowTranslucency_*); SmoothTiles and Copy are shared, Copy sees which one
+    // it serves from the format of the history texture (p.texBytes)
+    const bool translucent = p.kind.translucent;
+    Bindings b(p);
+    if (p.kind.pass == Pass::ClassifyTiles)
     {
         SigmaTilesArgs a;
-        a.z = p.tex[0]; a.penumbra = p.tex[1];
-        if (translucent) a.translucency = p.tex[2];
-        a.tiles = p.tex[translucent ? 3 : 2];
+        a.z = b.Next(); a.penumbra = b.Next(); a.translucency = b.Next(translucent); a.tiles = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.viewZScale = c.gViewZScale; a.denoisingRange = c.gDenoisingRange; a.unproject = c.gUnproject; a.orthoMode = c.gOrthoMode;
         a.tilesW = p.gridW; a.tilesH = p.gridH;
         int warps = a.tilesW * a.tilesH;
         if (translucent) NRD_B200_LAUNCH(p, (warps * 32 + 255) / 256, 256, a, SigmaClassifyTilesKernel<true>);
         else NRD_B200_LAUNCH(p, (warps * 32 + 255) / 256, 256, a, SigmaClassifyTilesKernel<false>);
     }
-    else if (!strcmp(shader, "SIGMA_SmoothTiles.cs"))
+    else if (p.kind.pass == Pass::SmoothTiles)
     {
         SigmaSmoothArgs a;
-        a.tiles = p.tex[0]; a.smoothed = p.tex[1];
+        a.tiles = b.Next(); a.smoothed = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.tilesMaxX = c.gTilesSizeMinusOne[0]; a.tilesMaxY = c.gTilesSizeMinusOne[1];
         NRD_B200_LAUNCH(p, dim3(p.gridW, p.gridH), dim3(16, 16), a, SigmaSmoothTilesKernel);
     }
-    else if (!strcmp(shader, "SIGMA_Copy.cs"))
+    else if (p.kind.pass == Pass::Copy)
     {
         SigmaCopyArgs a;
-        a.tiles = p.tex[0]; a.inHistory = p.tex[1]; a.inLength = p.tex[2]; a.outHistory = p.tex[3]; a.outLength = p.tex[4];
+        a.tiles = b.Next(); a.inHistory = b.Next(); a.inLength = b.Next(); a.outHistory = b.Next(); a.outLength = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.w = a.inHistory.w; a.h = a.inHistory.h; a.isRectChanged = c.gIsRectChanged; a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         const dim3 grid((a.w + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8), block(32, 8);
         if (p.preloadOnly || p.texBytes[3] == 4) NRD_B200_LAUNCH(p, grid, block, a, SigmaCopyKernel<true>);
         if (p.preloadOnly || p.texBytes[3] != 4) NRD_B200_LAUNCH(p, grid, block, a, SigmaCopyKernel<false>);
     }
-    else if (!strcmp(pass, "Blur.cs") || !strcmp(pass, "PostBlur.cs"))
+    else if (p.kind.pass == Pass::Blur || p.kind.pass == Pass::PostBlur)
     {
-        const bool first = !strcmp(pass, "Blur.cs");
-        const bool hasShadowInput = !first || translucent; // SIGMA_Blur.resources.hlsli:25-27
+        const bool first = p.kind.pass == Pass::Blur;
         SigmaBlurArgs a;
         a.c = c;
-        a.z = p.tex[0]; a.nr = p.tex[1]; a.penumbra = p.tex[2]; a.tiles = p.tex[3];
-        if (hasShadowInput) a.shadow = p.tex[4];
-        a.outPenumbra = p.tex[hasShadowInput ? 5 : 4];
-        a.outShadow = p.tex[hasShadowInput ? 6 : 5];
+        a.z = b.Next(); a.nr = b.Next(); a.penumbra = b.Next(); a.tiles = b.Next();
+        a.shadow = b.Next(!first || translucent); // SIGMA_Blur.resources.hlsli:25-27
+        a.outPenumbra = b.Next(); a.outShadow = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         dim3 grid((W + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8), block(32, 8);
         if (first && translucent) NRD_B200_LAUNCH(p, grid, block, a, SigmaBlurKernel<true, true>);
@@ -557,12 +557,13 @@ cudaError_t LaunchSigma(const PassLaunch& p, const char* shader)
         else if (translucent) NRD_B200_LAUNCH(p, grid, block, a, SigmaBlurKernel<false, true>);
         else NRD_B200_LAUNCH(p, grid, block, a, SigmaBlurKernel<false, false>);
     }
-    else if (!strcmp(pass, "TemporalStabilization.cs"))
+    else if (p.kind.pass == Pass::TemporalStabilization)
     {
         SigmaTsArgs a;
         a.c = c;
-        a.z = p.tex[0]; a.mv = p.tex[1]; a.penumbra = p.tex[2]; a.shadow = p.tex[3]; a.history = p.tex[4]; a.historyLength = p.tex[5]; a.tiles = p.tex[6];
-        a.outShadow = p.tex[7]; a.outLength = p.tex[8];
+        a.z = b.Next(); a.mv = b.Next(); a.penumbra = b.Next(); a.shadow = b.Next(); a.history = b.Next(); a.historyLength = b.Next(); a.tiles = b.Next();
+        a.outShadow = b.Next(); a.outLength = b.Next();
+        if (!b.Complete()) return cudaErrorInvalidValue;
         a.rowBegin = p.rowBegin; a.rowEnd = p.rowEnd;
         const dim3 grid((W + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8), block(32, 8);
         if (translucent) NRD_B200_LAUNCH(p, grid, block, a, SigmaTemporalStabilizationKernel<true>);

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../passes.h"
+
 namespace nrdb200_abi
 {
 constexpr int kMaxPeers = 8;
@@ -39,6 +41,7 @@ struct Surf
 // Launch bookkeeping handed from the executor to the launchers
 struct PassLaunch
 {
+    PassKind kind;         // the pipeline's pass (scheduler.h PipelineKind): picks the launcher, the kernel and the binding layout
     const void* constants; // host pointer to the dispatch's constant block
     uint32_t constantsSize;
     Surf tex[32];          // bindings in DispatchDesc order
@@ -48,7 +51,6 @@ struct PassLaunch
     int rowBegin, rowEnd;  // rows this launch must produce, in the pass's own pixel units
     cudaStream_t stream;
     bool preloadOnly;      // do not launch: only make the driver load the kernel this pass maps to (see NRD_B200_LAUNCH)
-    bool performanceMode;  // REBLUR: the pass is the "REBLUR_Perf_*" permutation (ReblurSettings::enablePerformanceMode)
     // Decoded-guide surface (executor-owned RGBA32F, not part of the DispatchDesc): {N.x, N.y, N.z, viewZ (REBLUR: unpacked |z * gViewZScale|, RELAX: raw)} of the current
     // frame's IN_NORMAL_ROUGHNESS / IN_VIEWZ.  guideMode 1 = this pass writes it (REBLUR ClassifyTiles, the first pass of every
     // frame; guideNr = IN_NORMAL_ROUGHNESS, which that dispatch does not bind itself), 2 = it is complete and the filter passes

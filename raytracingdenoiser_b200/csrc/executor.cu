@@ -22,7 +22,6 @@
 using namespace nrd;
 using namespace nrdb200;
 
-NRD_B200_DECLARE_LAUNCHERS(nrdb200_single)
 namespace nrdb200
 {
 cudaError_t LaunchClear(const PassLaunch& p);
@@ -30,28 +29,6 @@ cudaError_t LaunchClear(const PassLaunch& p);
 
 namespace
 {
-// the two builds of the kernels (device/common.cuh): one-GPU contexts never pay for the strip addressing
-struct Launchers
-{
-    cudaError_t (*classifyTiles)(const PassLaunch&);
-    cudaError_t (*hitDistReconstruction)(const PassLaunch&, int, bool);
-    cudaError_t (*prePass)(const PassLaunch&, int);
-    cudaError_t (*temporalAccumulation)(const PassLaunch&, int);
-    cudaError_t (*historyFix)(const PassLaunch&, int);
-    cudaError_t (*blur)(const PassLaunch&, int);
-    cudaError_t (*postBlur)(const PassLaunch&, int, bool);
-    cudaError_t (*temporalStabilization)(const PassLaunch&, int);
-    cudaError_t (*sigma)(const PassLaunch&, const char*);
-    cudaError_t (*relax)(const PassLaunch&, const char*);
-    cudaError_t (*aux)(const PassLaunch&, const char*); // split-screen passes, REFERENCE denoiser
-};
-const Launchers kStripLaunchers = {nrdb200::LaunchReblurClassifyTiles, nrdb200::LaunchReblurHitDistReconstruction, nrdb200::LaunchReblurPrePass, nrdb200::LaunchReblurTemporalAccumulation,
-                                   nrdb200::LaunchReblurHistoryFix, nrdb200::LaunchReblurBlur, nrdb200::LaunchReblurPostBlur,
-                                   nrdb200::LaunchReblurTemporalStabilization, nrdb200::LaunchSigma, nrdb200::LaunchRelax, nrdb200::LaunchAux};
-const Launchers kSingleLaunchers = {nrdb200_single::LaunchReblurClassifyTiles, nrdb200_single::LaunchReblurHitDistReconstruction, nrdb200_single::LaunchReblurPrePass, nrdb200_single::LaunchReblurTemporalAccumulation,
-                                    nrdb200_single::LaunchReblurHistoryFix, nrdb200_single::LaunchReblurBlur, nrdb200_single::LaunchReblurPostBlur,
-                                    nrdb200_single::LaunchReblurTemporalStabilization, nrdb200_single::LaunchSigma, nrdb200_single::LaunchRelax, nrdb200_single::LaunchAux};
-
 std::atomic<uint64_t> g_launchCount{0};
 std::mutex g_slotMutex;
 bool g_slotUsed[kMaxPeerSlots] = {};
@@ -344,66 +321,23 @@ Result UpdateRoughnessLut(NrdCudaContext* ctx, const float* hitDistParams, cudaS
     return Result::SUCCESS;
 }
 
-// "REBLUR_DiffuseSpecular_Blur.cs" -> family REBLUR, signal 2, pass "Blur"
-bool ParseReblur(const char* name, int& signal, const char*& pass, bool& perf)
-{
-    if (strncmp(name, "REBLUR_", 7) != 0) return false;
-    perf = !strncmp(name, "REBLUR_Perf_", 12); // ReblurSettings::enablePerformanceMode permutations (Source/Reblur.cpp:106-118)
-    const char* p = name + (perf ? 12 : 7);
-    if (!strncmp(p, "DiffuseSpecular_", 16)) { signal = 2; p += 16; }
-    else if (!strncmp(p, "Diffuse_", 8)) { signal = 0; p += 8; }
-    else if (!strncmp(p, "Specular_", 9)) { signal = 1; p += 9; }
-    else return false;
-    pass = p;
-    return true;
-}
-
-// pass (shader file name) -> kernel launcher of one build
-cudaError_t LaunchByName(const Launchers& L, const PassLaunch& launch, const char* shader)
-{
-    int signal = 0;
-    const char* pass = nullptr;
-    bool perf = false;
-    PassLaunch p = launch;
-    if (!strncmp(shader, "Clear_", 6)) return p.preloadOnly ? cudaSuccess : LaunchClear(p);
-    if (p.rowEnd <= p.rowBegin) return cudaSuccess; // a rank without rows still takes part in the barriers
-    if (strstr(shader, "_SplitScreen.cs") || !strncmp(shader, "REFERENCE_", 10)) return L.aux(p, shader);
-    if (!strcmp(shader, "REBLUR_ClassifyTiles.cs")) return L.classifyTiles(p);
-    if (ParseReblur(shader, signal, pass, perf))
-    {
-        p.performanceMode = perf;
-        if (!strcmp(pass, "HitDistReconstruction.cs")) return L.hitDistReconstruction(p, signal, false);
-        if (!strcmp(pass, "HitDistReconstruction_5x5.cs")) return L.hitDistReconstruction(p, signal, true);
-        if (!strcmp(pass, "PrePass.cs")) return L.prePass(p, signal);
-        if (!strcmp(pass, "TemporalAccumulation.cs")) return L.temporalAccumulation(p, signal);
-        if (!strcmp(pass, "HistoryFix.cs")) return L.historyFix(p, signal);
-        if (!strcmp(pass, "Blur.cs")) return L.blur(p, signal);
-        if (!strcmp(pass, "PostBlur.cs")) return L.postBlur(p, signal, false);
-        if (!strcmp(pass, "PostBlur_NoTemporalStabilization.cs")) return L.postBlur(p, signal, true);
-        if (!strcmp(pass, "TemporalStabilization.cs")) return L.temporalStabilization(p, signal);
-        return cudaErrorNotSupported;
-    }
-    if (!strncmp(shader, "SIGMA_", 6)) return L.sigma(p, shader);
-    if (!strncmp(shader, "RELAX_", 6)) return L.relax(p, shader);
-    return cudaErrorNotSupported;
-}
-
 // Loads every kernel the instance's pipelines map to (see NRD_B200_LAUNCH): nothing may be loaded lazily once barriers spin.
-void PreloadKernels(const NrdCudaContext* ctx, const Launchers& L)
+void PreloadKernels(const NrdCudaContext* ctx, cudaError_t (*launchPass)(const PassLaunch&))
 {
     alignas(16) static unsigned char dummy[1024] = {}; // a zeroed constant block big enough for every denoiser
     ((RelaxConstants*)dummy)->gDiffCheckerboard = ((RelaxConstants*)dummy)->gSpecCheckerboard = 2; // (checkerboard off; in preload mode every variant is loaded anyway)
-    const InstanceDesc& id = GetInstanceDesc(*ctx->instance);
-    for (uint32_t i = 0; i < id.pipelinesNum; i++)
+    const Scheduler& scheduler = *(const Scheduler*)ctx->instance;
+    for (uint32_t i = 0; i < scheduler.GetDesc().pipelinesNum; i++)
     {
         PassLaunch p{};
+        p.kind = scheduler.PipelineKind(i);
         p.constants = dummy;
         p.constantsSize = sizeof(dummy);
         p.gridW = p.gridH = 1;
         p.rowBegin = 0;
         p.rowEnd = 16;
         p.preloadOnly = true;
-        (void)LaunchByName(L, p, id.pipelines[i].shaderFileName); // passes without a kernel are reported when they are dispatched
+        (void)launchPass(p); // passes without a kernel are reported when they are dispatched
     }
 }
 
@@ -850,17 +784,12 @@ NRD_API Result nrdCudaConnectPeers(NrdCudaContext* ctx, uint32_t rank, uint32_t 
     for (uint32_t i = 0; i < (uint32_t)kMaxPeers; i++) table.delta[i] = ctx->peerDelta[i];
     for (uint32_t i = 0; i <= (uint32_t)kMaxPeers; i++) table.start[i] = i <= worldSize ? (int)ctx->stripStart[i] : 0x7fffffff;
     if (worldSize < (uint32_t)kMaxPeers) table.start[worldSize] = 0x7fffffff; // rows >= start[world] do not exist: never counted as an owner change
-    cudaError_t e = SetPeerTableReblurSpatial(ctx->peerSlot, &table);
-    if (e == cudaSuccess) e = SetPeerTableReblurHitDist(ctx->peerSlot, &table);
-    if (e == cudaSuccess) e = SetPeerTableReblurTemporal(ctx->peerSlot, &table);
-    if (e == cudaSuccess) e = SetPeerTableSigma(ctx->peerSlot, &table);
-    if (e == cudaSuccess) e = SetPeerTableRelax(ctx->peerSlot, &table);
-    if (e == cudaSuccess) e = SetPeerTableAux(ctx->peerSlot, &table);
+    cudaError_t e = SetPeerTables(ctx->peerSlot, &table);
     if (e != cudaSuccess) return Fail(ctx, Result::FAILURE, std::string("peer table: ") + cudaGetErrorString(e));
     ctx->rank = rank;
     ctx->world = worldSize;
     ctx->connected = true;
-    PreloadKernels(ctx, worldSize > 1 ? kStripLaunchers : kSingleLaunchers);
+    PreloadKernels(ctx, worldSize > 1 ? nrdb200::LaunchPass : nrdb200_single::LaunchPass);
     PreloadExecutorKernels();
     return Result::SUCCESS;
 }
@@ -917,6 +846,7 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     const InstanceDesc& id = GetInstanceDesc(*ctx->instance);
     if (d->pipelineIndex >= id.pipelinesNum) return Result::INVALID_ARGUMENT;
     const char* shader = id.pipelines[d->pipelineIndex].shaderFileName;
+    const PassKind kind = ((Scheduler*)ctx->instance)->PipelineKind(d->pipelineIndex);
     const CommonSettings& cs = ((Scheduler*)ctx->instance)->Common();
     // Dynamic resolution (Source/InstanceImpl.cpp:834-856, Shaders/Include/Common.hlsli:200-222): the passes run over rectSize <= resourceSize;
     // the application's guide inputs are addressed at rectOrigin + pixel (WithRectOrigin), everything else at the pixel itself.
@@ -931,6 +861,7 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
         return Fail(ctx, Result::FAILURE, "strip-mode context used before nrdCudaConnectPeers");
 
     PassLaunch p{};
+    p.kind = kind;
     p.constants = d->constantBufferData;
     p.constantsSize = d->constantBufferDataSize;
     p.texNum = d->resourcesNum;
@@ -949,9 +880,9 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     // checkerboarded REBLUR inputs (ReblurSettings::checkerboardMode) bind the same passes: the pre-pass resolves them, temporal
     // accumulation slows down on resolved pixels; RELAX and the split-screen passes reject them in their launchers
     // decoded-guide surface: ClassifyTiles (first pass of every REBLUR frame) fills it, all later passes of the frame read it
-    const bool isReblur = !strncmp(shader, "REBLUR_", 7), isRelax = !strncmp(shader, "RELAX_", 6);
-    const bool buildsGuide = !strcmp(shader, "REBLUR_ClassifyTiles.cs") || !strcmp(shader, "RELAX_ClassifyTiles.cs");
-    const bool isSplitScreen = strstr(shader, "_SplitScreen.cs") != nullptr; // may be the only pass of the frame (splitScreen >= 1)
+    const bool isReblur = kind.family == Family::REBLUR, isRelax = kind.family == Family::RELAX, isClear = kind.family == Family::CLEAR;
+    const bool buildsGuide = (isReblur || isRelax) && kind.pass == Pass::ClassifyTiles;
+    const bool isSplitScreen = kind.pass == Pass::SplitScreen; // may be the only pass of the frame (splitScreen >= 1)
     const bool readsGuide = (isReblur || isRelax) && !buildsGuide && !isSplitScreen; // every other REBLUR / RELAX pass reads it (REBLUR: and the roughness table)
     p.guide = ToSurf(ctx, ctx->guide);
     if (buildsGuide)
@@ -993,11 +924,10 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     // NRD_B200_FORCE_STRIP_KERNELS: run a one-GPU context on the strip build of the kernels.  The two builds are compiled
     // separately and differ in the last bits (FMA contraction); N-GPU results are bit-identical to THIS configuration.
     const bool stripBuild = (StripMode(ctx) && ctx->world > 1) || getenv("NRD_B200_FORCE_STRIP_KERNELS") != nullptr;
-    const Launchers& L = stripBuild ? kStripLaunchers : kSingleLaunchers;
     cudaError_t e;
-    const bool timed = ctx->timing && ctx->timingCount < 64 && strncmp(shader, "Clear_", 6) != 0;
+    const bool timed = ctx->timing && ctx->timingCount < 64 && !isClear;
     const uint32_t slot = ctx->timingCount;
-    const Texture* clearTarget = !strncmp(shader, "Clear_", 6) && d->resourcesNum ? Resolve(ctx, d->resources[0].type, d->resources[0].indexInPool) : nullptr;
+    const Texture* clearTarget = isClear && d->resourcesNum ? Resolve(ctx, d->resources[0].type, d->resources[0].indexInPool) : nullptr;
     if (clearTarget && !clearTarget->owned)
     {
         // an application texture (IN_MV / OUT_* are storage outputs of some passes): its pitch may exceed the row and the bytes
@@ -1006,10 +936,12 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
                                                   (cudaStream_t)stream)
                               : cudaSuccess;
     }
+    else if (isClear)
+        e = LaunchClear(p);
     else
     {
         if (timed) cudaEventRecord(ctx->timingEvents[3 * slot + 0], p.stream);
-        e = LaunchByName(L, p, shader);
+        e = stripBuild ? nrdb200::LaunchPass(p) : nrdb200_single::LaunchPass(p);
         if (timed) cudaEventRecord(ctx->timingEvents[3 * slot + 1], p.stream);
     }
 
@@ -1019,7 +951,7 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     if (buildsGuide) ctx->guideValid = true;
     const Texture* list[33];
     uint32_t n = 0;
-    if (strncmp(shader, "Clear_", 6) != 0 && pushMask) // clears zero the ghost rows locally
+    if (!isClear && pushMask) // clears zero the ghost rows locally
     {
         for (uint32_t i = 0; i < d->resourcesNum; i++)
             if ((pushMask >> i) & 1u) list[n++] = Resolve(ctx, d->resources[i].type, d->resources[i].indexInPool);

@@ -6,8 +6,6 @@
 #include "scheduler.h"
 
 #include <algorithm>
-#include <cstdio>
-#include <cstring>
 
 using namespace nrd;
 
@@ -33,21 +31,6 @@ enum ReblurPass : uint32_t
     RB_VALIDATION = RB_SPLIT_SCREEN + 1,
 };
 
-// shader file names are "<REBLUR|REBLUR_Perf>_<Diffuse|Specular|DiffuseSpecular>_<Pass>.cs"; they have to outlive the
-// instance, so they are interned once per process
-const char* ShaderName(bool perf, int signal, const char* pass)
-{
-    static char table[3][2][16][80];
-    static int used[3][2];
-    static const char* signalNames[3] = {"Diffuse", "Specular", "DiffuseSpecular"};
-    char tmp[80];
-    snprintf(tmp, sizeof(tmp), "%s_%s_%s.cs", perf ? "REBLUR_Perf" : "REBLUR", signalNames[signal], pass);
-    for (int i = 0; i < used[signal][perf]; i++)
-        if (!strcmp(table[signal][perf][i], tmp)) return table[signal][perf][i];
-    char* dst = table[signal][perf][used[signal][perf]++];
-    strcpy(dst, tmp);
-    return dst;
-}
 } // namespace
 
 void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
@@ -55,9 +38,14 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     new (&slot.settings.reblur) ReblurSettings();
     slot.settingsSize = sizeof(ReblurSettings);
 
-    const int signal = hasDiff && hasSpec ? 2 : (hasSpec ? 1 : 0);
-    const char* denoiserName = signal == 2 ? "REBLUR_DiffuseSpecular" : (signal == 1 ? "REBLUR_Specular" : "REBLUR_Diffuse");
+    const uint8_t signals = (hasDiff ? SIGNAL_DIFFUSE : 0) | (hasSpec ? SIGNAL_SPECULAR : 0);
+    const char* denoiserName = hasDiff && hasSpec ? "REBLUR_DiffuseSpecular" : (hasSpec ? "REBLUR_Specular" : "REBLUR_Diffuse");
     const uint32_t cb = sizeof(ReblurConstants);
+    // a pass and its performance-mode twin
+    auto EmitPair = [&](Pass pass) {
+        Emit({Family::REBLUR, pass, signals}, 8, 16, cb);
+        Emit({Family::REBLUR, pass, signals, true}, 8, 16, cb);
+    };
 
     // ---- permanent pool (Reblur_DiffuseSpecular.hpp:22-51, Reblur_Diffuse.hpp:20-37, Reblur_Specular.hpp:20-45)
     uint16_t next = kPermanentBase;
@@ -86,7 +74,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     next = kTransientBase;
     const uint16_t T_DATA1 = next++;
     const uint16_t T_DATA2 = next++;
-    AddTransient(signal == 2 ? Format::RG8_UNORM : Format::R8_UNORM);
+    AddTransient(hasDiff && hasSpec ? Format::RG8_UNORM : Format::R8_UNORM);
     AddTransient(hasSpec ? Format::R32_UINT : Format::R8_UINT);
     uint16_t T_HITDIST = 0, T_DIFF_TMP2 = 0, T_DIFF_FAST = 0, T_SPEC_TMP2 = 0, T_SPEC_FAST = 0;
     if (hasSpec) { T_HITDIST = next++; AddTransient(Format::R16_SFLOAT); }
@@ -103,7 +91,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     BeginPass(denoiserName, "Classify tiles");
     In(R(ResourceType::IN_VIEWZ));
     Out(T_TILES);
-    Emit("REBLUR_ClassifyTiles.cs", 16, 16, cb);
+    Emit({Family::REBLUR, Pass::ClassifyTiles}, 16, 16, cb); // shared by the three REBLUR denoisers
 
     for (int i = 0; i < 4; i++)
     {
@@ -114,9 +102,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
         if (hasSpec) In(IN_SPEC);
         if (hasDiff) Out(prepassEnabled ? DIFF_TEMP2 : DIFF_TEMP1);
         if (hasSpec) Out(prepassEnabled ? SPEC_TEMP2 : SPEC_TEMP1);
-        const char* pass = is5x5 ? "HitDistReconstruction_5x5" : "HitDistReconstruction";
-        Emit(ShaderName(false, signal, pass), 8, 16, cb);
-        Emit(ShaderName(true, signal, pass), 8, 16, cb);
+        EmitPair(is5x5 ? Pass::HitDistReconstruction_5x5 : Pass::HitDistReconstruction);
     }
 
     for (int i = 0; i < 2; i++)
@@ -128,8 +114,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
         if (hasSpec) In(afterReconstruction ? SPEC_TEMP2 : IN_SPEC);
         if (hasDiff) Out(DIFF_TEMP1);
         if (hasSpec) { Out(SPEC_TEMP1); Out(T_HITDIST); }
-        Emit(ShaderName(false, signal, "PrePass"), 8, 16, cb);
-        Emit(ShaderName(true, signal, "PrePass"), 8, 16, cb);
+        EmitPair(Pass::PrePass);
     }
 
     for (int i = 0; i < 8; i++)
@@ -143,7 +128,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
         if (hasSpec) In(hasConfidence ? R(ResourceType::IN_SPEC_CONFIDENCE) : kDummy);
         if (hasDiff) In(afterPrepass ? DIFF_TEMP1 : IN_DIFF);
         if (hasSpec) In(afterPrepass ? SPEC_TEMP1 : IN_SPEC);
-        if (signal == 2) { In(P_DIFF_HISTORY); In(P_SPEC_HISTORY); In(P_DIFF_FAST); In(P_SPEC_FAST); }
+        if (hasDiff && hasSpec) { In(P_DIFF_HISTORY); In(P_SPEC_HISTORY); In(P_DIFF_FAST); In(P_SPEC_FAST); }
         else if (hasDiff) { In(P_DIFF_HISTORY); In(P_DIFF_FAST); }
         else { In(P_SPEC_HISTORY); In(P_SPEC_FAST); }
         if (hasSpec) { In(P_HITDIST_PING, P_HITDIST_PONG); In(T_HITDIST); }
@@ -152,8 +137,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
         if (hasDiff) Out(T_DIFF_FAST);
         if (hasSpec) { Out(T_SPEC_FAST); Out(P_HITDIST_PONG, P_HITDIST_PING); }
         Out(T_DATA1); Out(T_DATA2);
-        Emit(ShaderName(false, signal, "TemporalAccumulation"), 8, 16, cb);
-        Emit(ShaderName(true, signal, "TemporalAccumulation"), 8, 16, cb);
+        EmitPair(Pass::TemporalAccumulation);
     }
 
     BeginPass(denoiserName, "History fix");
@@ -166,8 +150,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     if (hasSpec) Out(SPEC_TEMP1);
     if (hasDiff) Out(P_DIFF_FAST);
     if (hasSpec) Out(P_SPEC_FAST);
-    Emit(ShaderName(false, signal, "HistoryFix"), 8, 16, cb);
-    Emit(ShaderName(true, signal, "HistoryFix"), 8, 16, cb);
+    EmitPair(Pass::HistoryFix);
 
     BeginPass(denoiserName, "Blur");
     In(T_TILES); In(R(ResourceType::IN_NORMAL_ROUGHNESS)); In(T_DATA1);
@@ -177,8 +160,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     if (hasDiff) Out(DIFF_TEMP2);
     if (hasSpec) Out(SPEC_TEMP2);
     Out(P_PREV_VIEWZ);
-    Emit(ShaderName(false, signal, "Blur"), 8, 16, cb);
-    Emit(ShaderName(true, signal, "Blur"), 8, 16, cb);
+    EmitPair(Pass::Blur);
 
     for (int i = 0; i < 2; i++)
     {
@@ -197,9 +179,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
             if (hasDiff) Out(R(ResourceType::OUT_DIFF_RADIANCE_HITDIST));
             if (hasSpec) Out(R(ResourceType::OUT_SPEC_RADIANCE_HITDIST));
         }
-        const char* pass = withStabilization ? "PostBlur" : "PostBlur_NoTemporalStabilization";
-        Emit(ShaderName(false, signal, pass), 8, 16, cb);
-        Emit(ShaderName(true, signal, pass), 8, 16, cb);
+        EmitPair(withStabilization ? Pass::PostBlur : Pass::PostBlur_NoTemporalStabilization);
     }
 
     for (int i = 0; i < 2; i++)
@@ -219,8 +199,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
         if (hasSpec) Out(R(ResourceType::OUT_SPEC_RADIANCE_HITDIST));
         if (hasDiff) Out(P_DIFF_STAB_PONG, P_DIFF_STAB_PING);
         if (hasSpec) Out(P_SPEC_STAB_PONG, P_SPEC_STAB_PING);
-        Emit(ShaderName(false, signal, "TemporalStabilization"), 8, 16, cb);
-        Emit(ShaderName(true, signal, "TemporalStabilization"), 8, 16, cb);
+        EmitPair(Pass::TemporalStabilization);
     }
 
     BeginPass(denoiserName, "Split screen");
@@ -229,7 +208,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     if (hasSpec) In(IN_SPEC);
     if (hasDiff) Out(R(ResourceType::OUT_DIFF_RADIANCE_HITDIST));
     if (hasSpec) Out(R(ResourceType::OUT_SPEC_RADIANCE_HITDIST));
-    Emit(ShaderName(false, signal, "SplitScreen"), 8, 16, cb);
+    Emit({Family::REBLUR, Pass::SplitScreen, signals}, 8, 16, cb);
 
     BeginPass(denoiserName, "Validation");
     In(R(ResourceType::IN_NORMAL_ROUGHNESS)); In(R(ResourceType::IN_VIEWZ)); In(R(ResourceType::IN_MV)); In(T_DATA1); In(T_DATA2);
@@ -237,7 +216,7 @@ void Scheduler::AddReblur(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     In(hasDiff ? IN_DIFF : IN_SPEC);
     In(hasSpec ? IN_SPEC : IN_DIFF);
     Out(R(ResourceType::OUT_VALIDATION));
-    Emit("REBLUR_Validation.cs", 8, 16, cb + 8, kIgnoreRect); // + gHasDiffuse, gHasSpecular (840 = sizeof of the reference struct)
+    Emit({Family::REBLUR, Pass::Validation}, 8, 16, cb + 8, kIgnoreRect); // + gHasDiffuse, gHasSpecular (840 = sizeof of the reference struct)
 }
 
 void Scheduler::UpdateReblur(const DenoiserSlot& slot)

@@ -27,12 +27,12 @@ void Scheduler::AddReference(DenoiserSlot& slot)
     BeginPass(dn, "Temporal accumulation");
     In(R(ResourceType::IN_SIGNAL));
     Out(P_HISTORY);
-    Emit("REFERENCE_TemporalAccumulation.cs", 16, 16, sizeof(ReferenceAccumulateConstants));
+    Emit({Family::REFERENCE, Pass::TemporalAccumulation}, 16, 16, sizeof(ReferenceAccumulateConstants));
 
     BeginPass(dn, "Copy");
     In(P_HISTORY);
     Out(R(ResourceType::OUT_SIGNAL));
-    Emit("REFERENCE_Copy.cs", 16, 16, sizeof(ReferenceCopyConstants));
+    Emit({Family::REFERENCE, Pass::Copy}, 16, 16, sizeof(ReferenceCopyConstants));
 }
 
 void Scheduler::UpdateReference(const DenoiserSlot& slot)

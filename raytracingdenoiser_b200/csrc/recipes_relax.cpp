@@ -5,7 +5,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
 #include <cstring>
 
 using namespace nrd;
@@ -37,22 +36,6 @@ enum RelaxPass : uint32_t
 const uint32_t kSharedSize = offsetof(RelaxConstants, gStepSize); // 704
 } // namespace
 
-// shader file names are "RELAX_<Diffuse|Specular|DiffuseSpecular>_<Pass>.cs"; they have to outlive the instance, so they are
-// interned once per process
-static const char* RelaxShaderName(int signal, const char* pass)
-{
-    static char table[3][16][80];
-    static int used[3];
-    static const char* signalNames[3] = {"Diffuse", "Specular", "DiffuseSpecular"};
-    char tmp[80];
-    snprintf(tmp, sizeof(tmp), "RELAX_%s_%s.cs", signalNames[signal], pass);
-    for (int i = 0; i < used[signal]; i++)
-        if (!strcmp(table[signal][i], tmp)) return table[signal][i];
-    char* dst = table[signal][used[signal]++];
-    strcpy(dst, tmp);
-    return dst;
-}
-
 // One builder for Source/Denoisers/Relax_Diffuse.hpp, Relax_Specular.hpp and Relax_DiffuseSpecular.hpp: the one-signal graphs are
 // the two-signal graph without the other signal's textures and bindings (pool order: Relax_Diffuse.hpp:17-44, Relax_Specular.hpp:17-52,
 // Relax_DiffuseSpecular.hpp:17-62).
@@ -60,8 +43,8 @@ void Scheduler::AddRelax(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
 {
     new (&slot.settings.relax) RelaxSettings();
     slot.settingsSize = sizeof(RelaxSettings);
-    const int signal = hasDiff && hasSpec ? 2 : (hasSpec ? 1 : 0);
-    const char* dn = signal == 2 ? "RELAX_DiffuseSpecular" : (signal == 1 ? "RELAX_Specular" : "RELAX_Diffuse");
+    const uint8_t signals = (hasDiff ? SIGNAL_DIFFUSE : 0) | (hasSpec ? SIGNAL_SPECULAR : 0);
+    const char* dn = hasDiff && hasSpec ? "RELAX_DiffuseSpecular" : (hasSpec ? "RELAX_Specular" : "RELAX_Diffuse");
     const uint32_t cb = kSharedSize;
     const uint32_t cbAtrous = offsetof(RelaxConstants, gIsLastPass) + sizeof(uint32_t); // 712: sizeof() of the reference struct, no register padding
 
@@ -103,14 +86,14 @@ void Scheduler::AddRelax(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
     BeginPass(dn, "Classify tiles");
     In(VZ);
     Out(T_TILES);
-    Emit("RELAX_ClassifyTiles.cs", 16, 16, cb);
+    Emit({Family::RELAX, Pass::ClassifyTiles}, 16, 16, cb); // shared by the three RELAX denoisers
 
     for (int i = 0; i < 2; i++)
     {
         BeginPass(dn, "Hit distance reconstruction");
         In(T_TILES); InS(IN_SPEC); InD(IN_DIFF); In(NR); In(VZ);
         OutS(T_SPEC_ILLUM_PING); OutD(T_DIFF_ILLUM_PING);
-        Emit(RelaxShaderName(signal, i ? "HitDistReconstruction_5x5" : "HitDistReconstruction"), 8, 8, cb);
+        Emit({Family::RELAX, i ? Pass::HitDistReconstruction_5x5 : Pass::HitDistReconstruction, signals}, 8, 8, cb);
     }
 
     for (int i = 0; i < 2; i++)
@@ -118,7 +101,7 @@ void Scheduler::AddRelax(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
         BeginPass(dn, "Pre-pass");
         In(T_TILES); InS(i ? T_SPEC_ILLUM_PING : IN_SPEC); InD(i ? T_DIFF_ILLUM_PING : IN_DIFF); In(NR); In(VZ);
         OutS(OUT_SPEC); OutD(OUT_DIFF);
-        Emit(RelaxShaderName(signal, "PrePass"), 16, 16, cb);
+        Emit({Family::RELAX, Pass::PrePass, signals}, 16, 16, cb);
     }
 
     for (int i = 0; i < 4; i++)
@@ -134,28 +117,28 @@ void Scheduler::AddRelax(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
         In(hasMix ? R(ResourceType::IN_DISOCCLUSION_THRESHOLD_MIX) : kDummy);
         OutS(T_SPEC_ILLUM_PING); OutD(T_DIFF_ILLUM_PING); OutS(T_SPEC_ILLUM_PONG); OutD(T_DIFF_ILLUM_PONG);
         OutS(P_REFLECTION_HIT_T_CURR, P_REFLECTION_HIT_T_PREV); Out(T_HISTORY_LENGTH); OutS(T_SPEC_REPROJECTION_CONFIDENCE);
-        Emit(RelaxShaderName(signal, "TemporalAccumulation"), 8, 16, cb);
+        Emit({Family::RELAX, Pass::TemporalAccumulation, signals}, 8, 16, cb);
     }
 
     BeginPass(dn, "History fix");
     In(T_TILES); InS(T_SPEC_ILLUM_PING); InD(T_DIFF_ILLUM_PING); In(T_HISTORY_LENGTH); In(NR); In(VZ);
     OutS(T_SPEC_ILLUM_PONG); OutD(T_DIFF_ILLUM_PONG);
-    Emit(RelaxShaderName(signal, "HistoryFix"), 8, 8, cb);
+    Emit({Family::RELAX, Pass::HistoryFix, signals}, 8, 8, cb);
 
     BeginPass(dn, "History clamping");
     In(T_TILES); In(VZ); InS(OUT_SPEC); InD(OUT_DIFF); InS(T_SPEC_ILLUM_PING); InD(T_DIFF_ILLUM_PING); InS(T_SPEC_ILLUM_PONG); InD(T_DIFF_ILLUM_PONG); In(T_HISTORY_LENGTH);
     OutS(P_SPEC_ILLUM_PREV); OutD(P_DIFF_ILLUM_PREV); OutS(P_SPEC_ILLUM_RESPONSIVE_PREV); OutD(P_DIFF_ILLUM_RESPONSIVE_PREV); Out(P_HISTORY_LENGTH_PREV);
-    Emit(RelaxShaderName(signal, "HistoryClamping"), 8, 8, cb);
+    Emit({Family::RELAX, Pass::HistoryClamping, signals}, 8, 8, cb);
 
     BeginPass(dn, "Copy");
     InS(P_SPEC_ILLUM_PREV); InD(P_DIFF_ILLUM_PREV);
     OutS(OUT_SPEC); OutD(OUT_DIFF);
-    Emit(RelaxShaderName(signal, "Copy"), 8, 8, cb);
+    Emit({Family::RELAX, Pass::Copy, signals}, 8, 8, cb);
 
     BeginPass(dn, "Anti-firefly");
     In(T_TILES); InS(OUT_SPEC); InD(OUT_DIFF); In(NR); In(VZ);
     OutS(P_SPEC_ILLUM_PREV); OutD(P_DIFF_ILLUM_PREV);
-    Emit(RelaxShaderName(signal, "AntiFirefly"), 8, 8, cb);
+    Emit({Family::RELAX, Pass::AntiFirefly, signals}, 8, 8, cb);
 
     for (int i = 0; i < 2; i++)
     {
@@ -174,20 +157,20 @@ void Scheduler::AddRelax(DenoiserSlot& slot, bool hasDiff, bool hasSpec)
             else { OutS(isEven ? T_SPEC_ILLUM_PING : T_SPEC_ILLUM_PONG); OutD(isEven ? T_DIFF_ILLUM_PING : T_DIFF_ILLUM_PONG); }
             if (isSmem) { Out(P_NORMAL_ROUGHNESS_PREV); Out(P_MATERIAL_ID_PREV); Out(P_VIEWZ_PREV); }
             const uint16_t repeats = isLast ? 1 : (kMaxAtrousPasses - 2 + 1) / 2;
-            if (isSmem) Emit(RelaxShaderName(signal, "AtrousSmem"), 8, 8, cbAtrous);
-            else Emit(RelaxShaderName(signal, "Atrous"), 16, 16, cbAtrous, 1, repeats);
+            if (isSmem) Emit({Family::RELAX, Pass::AtrousSmem, signals}, 8, 8, cbAtrous);
+            else Emit({Family::RELAX, Pass::Atrous, signals}, 16, 16, cbAtrous, 1, repeats);
         }
     }
 
     BeginPass(dn, "Split screen");
     In(VZ); InD(IN_DIFF); InS(IN_SPEC);
     OutD(OUT_DIFF); OutS(OUT_SPEC);
-    Emit(RelaxShaderName(signal, "SplitScreen"), 8, 16, cb);
+    Emit({Family::RELAX, Pass::SplitScreen, signals}, 8, 16, cb);
 
     BeginPass(dn, "Validation");
     In(NR); In(VZ); In(R(ResourceType::IN_MV)); In(T_HISTORY_LENGTH);
     Out(R(ResourceType::OUT_VALIDATION));
-    Emit("RELAX_Validation.cs", 8, 16, cb, kIgnoreRect);
+    Emit({Family::RELAX, Pass::Validation}, 8, 16, cb, kIgnoreRect);
 }
 
 void Scheduler::UpdateRelax(const DenoiserSlot& slot)

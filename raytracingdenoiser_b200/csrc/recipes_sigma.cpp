@@ -24,17 +24,8 @@ void Scheduler::AddSigmaShadow(DenoiserSlot& slot, bool translucent)
     slot.settingsSize = sizeof(SigmaSettings);
     const char* dn = translucent ? "SIGMA_ShadowTranslucency" : "SIGMA_Shadow";
     const Format shadowFormat = translucent ? Format::RGBA8_UNORM : Format::R8_UNORM;
-    // "SIGMA_Shadow_<pass>.cs" / "SIGMA_ShadowTranslucency_<pass>.cs" (string literals: they outlive every instance)
-    static const char* const kNames[2][5] = {
-        {"SIGMA_Shadow_ClassifyTiles.cs", "SIGMA_Shadow_Blur.cs", "SIGMA_Shadow_PostBlur.cs", "SIGMA_Shadow_TemporalStabilization.cs", "SIGMA_Shadow_SplitScreen.cs"},
-        {"SIGMA_ShadowTranslucency_ClassifyTiles.cs", "SIGMA_ShadowTranslucency_Blur.cs", "SIGMA_ShadowTranslucency_PostBlur.cs",
-         "SIGMA_ShadowTranslucency_TemporalStabilization.cs", "SIGMA_ShadowTranslucency_SplitScreen.cs"}};
-    auto shader = [&](const char* pass) {
-        static const char* const passes[5] = {"ClassifyTiles", "Blur", "PostBlur", "TemporalStabilization", "SplitScreen"};
-        for (int i = 0; i < 5; i++)
-            if (!strcmp(pass, passes[i])) return kNames[translucent ? 1 : 0][i];
-        return (const char*)nullptr;
-    };
+    // "SIGMA_Shadow_<pass>.cs" / "SIGMA_ShadowTranslucency_<pass>.cs"; SmoothTiles and Copy are shared by both denoisers
+    auto kind = [&](Pass pass) { return PassKind{Family::SIGMA, pass, SIGNAL_SHADOW, false, translucent}; };
     // the reference reports sizeof() of its C++ struct, which has no tail padding to a 16-byte register (516, not 528)
     const uint32_t cb = offsetof(SigmaConstants, gIsRectChanged) + sizeof(uint32_t);
 
@@ -56,23 +47,23 @@ void Scheduler::AddSigmaShadow(DenoiserSlot& slot, bool translucent)
     In(R(ResourceType::IN_VIEWZ)); In(R(ResourceType::IN_PENUMBRA));
     if (translucent) In(R(ResourceType::IN_TRANSLUCENCY));
     Out(T_TILES);
-    Emit(shader("ClassifyTiles"), 16, 16, cb);
+    Emit(kind(Pass::ClassifyTiles), 16, 16, cb);
 
     BeginPass(dn, "Smooth tiles");
     In(T_TILES);
     Out(T_SMOOTHED_TILES);
-    Emit("SIGMA_SmoothTiles.cs", 16, 16, cb, 16);
+    Emit({Family::SIGMA, Pass::SmoothTiles}, 16, 16, cb, 16);
 
     BeginPass(dn, "Copy");
     In(T_SMOOTHED_TILES); In(R(ResourceType::OUT_SHADOW_TRANSLUCENCY)); In(P_HISTORY_LENGTH);
     Out(T_HISTORY); Out(T_HISTORY_LENGTH);
-    Emit("SIGMA_Copy.cs", 8, 16, cb, kUseMaxDims);
+    Emit({Family::SIGMA, Pass::Copy}, 8, 16, cb, kUseMaxDims);
 
     BeginPass(dn, "Blur");
     In(R(ResourceType::IN_VIEWZ)); In(R(ResourceType::IN_NORMAL_ROUGHNESS)); In(R(ResourceType::IN_PENUMBRA)); In(T_SMOOTHED_TILES);
     if (translucent) In(R(ResourceType::IN_TRANSLUCENCY));
     Out(T_DATA_1); Out(T_TEMP_1);
-    Emit(shader("Blur"), 8, 16, cb, translucent ? (uint16_t)1 : kUseMaxDims);
+    Emit(kind(Pass::Blur), 8, 16, cb, translucent ? (uint16_t)1 : kUseMaxDims);
 
     for (int i = 0; i < 2; i++)
     {
@@ -81,19 +72,19 @@ void Scheduler::AddSigmaShadow(DenoiserSlot& slot, bool translucent)
         In(R(ResourceType::IN_VIEWZ)); In(R(ResourceType::IN_NORMAL_ROUGHNESS)); In(T_DATA_1); In(T_SMOOTHED_TILES); In(T_TEMP_1);
         Out(T_DATA_2);
         Out(stabilized ? T_TEMP_2 : R(ResourceType::OUT_SHADOW_TRANSLUCENCY));
-        Emit(shader("PostBlur"), 8, 16, cb);
+        Emit(kind(Pass::PostBlur), 8, 16, cb);
     }
 
     BeginPass(dn, "Temporal stabilization");
     In(R(ResourceType::IN_VIEWZ)); In(R(ResourceType::IN_MV)); In(T_DATA_2); In(T_TEMP_2); In(T_HISTORY); In(T_HISTORY_LENGTH); In(T_SMOOTHED_TILES);
     Out(R(ResourceType::OUT_SHADOW_TRANSLUCENCY)); Out(P_HISTORY_LENGTH);
-    Emit(shader("TemporalStabilization"), 8, 16, cb);
+    Emit(kind(Pass::TemporalStabilization), 8, 16, cb);
 
     BeginPass(dn, "Split screen");
     In(R(ResourceType::IN_VIEWZ)); In(R(ResourceType::IN_PENUMBRA));
     if (translucent) In(R(ResourceType::IN_TRANSLUCENCY));
     Out(R(ResourceType::OUT_SHADOW_TRANSLUCENCY));
-    Emit(shader("SplitScreen"), 8, 16, cb);
+    Emit(kind(Pass::SplitScreen), 8, 16, cb);
 }
 
 void Scheduler::UpdateSigma(const DenoiserSlot& slot)

@@ -34,9 +34,9 @@ Scheduler::Scheduler(const MemoryHooks& hooks)
       transientPool_(HookAllocator<TextureDesc>(&hooks_)), resources_(HookAllocator<ResourceDesc>(&hooks_)),
       clears_(HookAllocator<ClearTarget>(&hooks_)), pingPongs_(HookAllocator<PingPong>(&hooks_)),
       ranges_(HookAllocator<ResourceRangeDesc>(&hooks_)), pipelineRangeOffset_(HookAllocator<size_t>(&hooks_)),
-      pipelines_(HookAllocator<PipelineDesc>(&hooks_)), passes_(HookAllocator<PassTemplate>(&hooks_)),
-      active_(HookAllocator<DispatchDesc>(&hooks_)), transientRemap_(HookAllocator<uint16_t>(&hooks_)),
-      ownedStrings_(HookAllocator<char*>(&hooks_))
+      pipelines_(HookAllocator<PipelineDesc>(&hooks_)), pipelineKinds_(HookAllocator<PassKind>(&hooks_)),
+      passes_(HookAllocator<PassTemplate>(&hooks_)), active_(HookAllocator<DispatchDesc>(&hooks_)),
+      transientRemap_(HookAllocator<uint16_t>(&hooks_)), ownedStrings_(HookAllocator<char*>(&hooks_))
 {
     constantArenaRaw_ = (uint8_t*)hooks_.alloc(kConstantArenaSize + 16, 16);
     constantArena_ = (uint8_t*)(((uintptr_t)constantArenaRaw_ + 15) & ~(uintptr_t)15);
@@ -135,13 +135,13 @@ Result Scheduler::Create(const InstanceCreationDesc& creation)
     passName_ = "Clear (f)";
     passResourceOffset_ = resources_.size();
     Out(0);
-    Emit("Clear_Float.cs", 16, 16, 0);
+    Emit({Family::CLEAR, Pass::Float}, 16, 16, 0);
 
     clearPass_[1] = passes_.size();
     passName_ = "Clear (ui)";
     passResourceOffset_ = resources_.size();
     Out(0);
-    Emit("Clear_Uint.cs", 16, 16, 0);
+    Emit({Family::CLEAR, Pass::Uint}, 16, 16, 0);
 
     FinalizeDesc();
     return Result::SUCCESS;
@@ -194,17 +194,36 @@ void Scheduler::PushResource(DescriptorType type, uint16_t localId, uint16_t swa
     resources_.push_back({type, resourceType, index});
 }
 
-void Scheduler::Emit(const char* shaderFileName, uint8_t threadsX, uint8_t threadsY, uint32_t constantSize, uint16_t downsample, uint16_t maxRepeats)
+// "<family>[_Perf][_<signals>]_<pass>.cs", e.g. REBLUR_Perf_DiffuseSpecular_Blur.cs, SIGMA_ShadowTranslucency_Blur.cs, Clear_Float.cs
+static void ShaderFileName(const PassKind& k, char* out, size_t size)
+{
+    static const char* const kFamilies[] = {"Clear", "REBLUR", "RELAX", "SIGMA", "REFERENCE"};
+#define NRD_B200_PASS_NAME(name) #name,
+    static const char* const kPasses[] = {NRD_B200_PASSES(NRD_B200_PASS_NAME)};
+#undef NRD_B200_PASS_NAME
+    static const char* const kSignals[] = {"", "Diffuse", "Specular", "DiffuseSpecular", "Shadow"};
+    const char* signal = k.translucent ? "ShadowTranslucency" : kSignals[k.signals];
+    snprintf(out, size, "%s%s%s%s_%s.cs", kFamilies[(int)k.family], k.perf ? "_Perf" : "", *signal ? "_" : "", signal, kPasses[(int)k.pass]);
+}
+
+void Scheduler::Emit(const PassKind& kind, uint8_t threadsX, uint8_t threadsY, uint32_t constantSize, uint16_t downsample, uint16_t maxRepeats)
 {
     // pipelines are unique per shader file name (reference: InstanceImpl.cpp:592-633)
+    char shaderFileName[80];
+    ShaderFileName(kind, shaderFileName, sizeof(shaderFileName));
     size_t pipelineIndex = 0;
     for (; pipelineIndex < pipelines_.size(); pipelineIndex++)
         if (!strcmp(pipelines_[pipelineIndex].shaderFileName, shaderFileName)) break;
 
     if (pipelineIndex == pipelines_.size())
     {
+        const size_t n = strlen(shaderFileName) + 1;
+        char* name = (char*)hooks_.alloc(n, 1);
+        memcpy(name, shaderFileName, n);
+        ownedStrings_.push_back(name);
+        pipelineKinds_.push_back(kind);
         PipelineDesc pd{};
-        pd.shaderFileName = shaderFileName;
+        pd.shaderFileName = name;
         pd.shaderEntryPointName = "main";
         pd.hasConstantData = constantSize != 0;
         pipelineRangeOffset_.push_back(ranges_.size());

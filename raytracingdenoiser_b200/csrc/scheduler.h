@@ -6,6 +6,7 @@
 #include "../../include/nrd_b200.h"
 #include "constants.h"
 #include "hostmath.h"
+#include "passes.h"
 
 #include <chrono>
 #include <new>
@@ -13,6 +14,8 @@
 
 namespace nrdb200
 {
+using namespace nrdb200_abi; // PassKind (passes.h)
+
 // STL allocator over the user's AllocationCallbacks (reference: Source/StdAllocator.h)
 struct MemoryHooks
 {
@@ -100,6 +103,7 @@ public:
     const nrd::InstanceDesc& GetDesc() const { return desc_; }
     const MemoryHooks& Hooks() const { return hooks_; }
     const nrd::CommonSettings& Common() const { return common_; }
+    const PassKind& PipelineKind(size_t pipelineIndex) const { return pipelineKinds_[pipelineIndex]; }
     bool HasDenoiser(nrd::Denoiser d) const
     {
         for (size_t i = 0; i < slots_.size(); i++)
@@ -113,7 +117,7 @@ public:
     void BeginPass(const char* denoiserName, const char* passName);
     void In(uint16_t localId, uint16_t swapWith = kNoSwap) { PushResource(nrd::DescriptorType::TEXTURE, localId, swapWith); }
     void Out(uint16_t localId, uint16_t swapWith = kNoSwap) { PushResource(nrd::DescriptorType::STORAGE_TEXTURE, localId, swapWith); }
-    void Emit(const char* shaderFileName, uint8_t threadsX, uint8_t threadsY, uint32_t constantSize, uint16_t downsample = 1, uint16_t maxRepeats = 1);
+    void Emit(const PassKind& kind, uint8_t threadsX, uint8_t threadsY, uint32_t constantSize, uint16_t downsample = 1, uint16_t maxRepeats = 1);
     void* Push(const DenoiserSlot& slot, uint32_t localPassIndex); // activates a pass for this frame, returns its constant block
 
     // ---- per-frame derived camera state (read by the recipes when they fill constants) ----
@@ -155,6 +159,7 @@ private:
     Vec<nrd::ResourceRangeDesc> ranges_;
     Vec<size_t> pipelineRangeOffset_;
     Vec<nrd::PipelineDesc> pipelines_;
+    Vec<PassKind> pipelineKinds_; // one per pipeline
     Vec<PassTemplate> passes_;
     Vec<nrd::DispatchDesc> active_;
     Vec<uint16_t> transientRemap_;
