@@ -84,7 +84,7 @@ static __device__ __forceinline__ const uint8_t* PeerRow(const Surf& s, int y)
 template <class T> __device__ __forceinline__ const T* TexelPtr(const Surf& s, int x, int y)
 {
 #if defined(NRD_B200_NO_STRIPS)
-    return reinterpret_cast<const T*>(s.base + (size_t)y * s.pitch) + x; // the whole texture is local: ly0 == 0 (executor.cu ToSurf)
+    return reinterpret_cast<const T*>(s.base + (size_t)y * s.pitch) + x; // the whole texture is local: ly0 == 0 (arena.cu Arena::ToSurf)
 #else
     const int ly = y - s.ly0;
     if (s.stripRows != 0 && (unsigned)ly >= s.lrows) return reinterpret_cast<const T*>(PeerRow(s, y)) + x;

@@ -21,7 +21,7 @@ struct PeerTable
 
 // A pitched HBM surface.  On one GPU the whole texture is local.  In strip mode (several GPUs, one horizontal strip
 // each) a surface holds its own strip plus `halo` ghost rows above and below, which the owner of those
-// rows refreshes after every pass that writes them (executor.cu, GhostPushKernel); a tap that lands outside even the
+// rows refreshes after every pass that writes them (arena.cu, GhostPushKernel); a tap that lands outside even the
 // ghost rows is loaded straight from the owner's HBM: every context carves its surfaces out of one arena with the same
 // layout, so that address is the local address plus (arena of the owner - local arena).  Stores are always local.
 struct Surf

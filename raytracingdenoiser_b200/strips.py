@@ -2,7 +2,7 @@
 
 Every rank runs the SAME pass list on its own strip (`nrd.CudaContext(strip=..., strip_height=...)`); rows of other strips
 are read by the kernels straight from the owner's HBM over NVLink (CUDA IPC mapping of the owner's arena), and a device-side
-flag barrier separates the passes (csrc/executor.cu).  There is no data-path collective: torch.distributed only carries the
+flag barrier separates the passes (csrc/arena.cu).  There is no data-path collective: torch.distributed only carries the
 64-byte IPC handles at start-up and the timing reductions of bench.py.
 """
 import os

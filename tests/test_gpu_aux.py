@@ -118,3 +118,38 @@ def test_user_textures_in_wider_formats_give_the_same_result():
         assert torch.equal(got, want[name].to(torch.float32)), name
     ctx.destroy()
     inst.destroy()
+
+
+@pytest.mark.parametrize("denoiser_name", ["REBLUR_DIFFUSE_SPECULAR", "SIGMA_SHADOW_TRANSLUCENCY"])
+def test_user_textures_and_formats_match_the_python_table(denoiser_name):
+    """The executor's user textures and their formats against harness.USER_FORMATS, which applications and bench.py read:
+    binding a user texture in its listed format succeeds exactly for the listed types (others are UNSUPPORTED), and a strip-mode
+    context that covers the whole frame holds exactly the listed textures, in that format."""
+    import torch
+    from raytracingdenoiser_b200 import harness, nrd
+    den = getattr(nrd.Denoiser, denoiser_name)
+    w, h = 64, 32
+    inst = nrd.Instance([(0, den)])
+    ctx = nrd.CudaContext(inst, w, h)
+    strip = nrd.CudaContext(inst, w, h, strip=(0, h), strip_height=h)
+    texels = torch.zeros((h, w, 16), dtype=torch.uint8, device="cuda")  # 16 bytes per texel: room for every format
+    try:
+        for rt in nrd.ResourceType:
+            if rt >= nrd.ResourceType.TRANSIENT_POOL:
+                continue
+            listed = rt.name in harness.USER_FORMATS
+            fmt = harness.user_format(den, rt.name)[0] if listed else nrd.Format.RGBA32_SFLOAT
+            if listed:
+                ctx.set_user_texture(rt, texels.data_ptr(), texels.stride(0), fmt)
+                info = strip.get_texture(rt)
+                assert (info.format, info.width, info.height, info.firstRow, info.rowsNum) == (int(fmt), w, h, 0, h), rt.name
+            else:
+                with pytest.raises(nrd.NrdError) as e:
+                    ctx.set_user_texture(rt, texels.data_ptr(), texels.stride(0), fmt)
+                assert e.value.result == nrd.Result.UNSUPPORTED, rt.name
+                with pytest.raises(nrd.NrdError):
+                    strip.get_texture(rt)
+    finally:
+        strip.destroy()
+        ctx.destroy()
+        inst.destroy()
