@@ -45,7 +45,10 @@ struct CatRomSetup
 __device__ __forceinline__ CatRomSetup SetupCatRom(f2 samplePos, const float* invSize, f4 customWeights, bool useBicubic)
 {
     CatRomSetup s;
-    float cx = floorf(samplePos.x - 0.5f) + 0.5f, cy = floorf(samplePos.y - 0.5f) + 0.5f;
+    // texel of the footprint's centre: floor, not a conversion to int, which rounds -0.5 (a sample within half a texel of the
+    // top or left edge) towards texel 0 instead of -1; the reference's sampler taps are placed at centerPos itself
+    const float x0 = floorf(samplePos.x - 0.5f), y0 = floorf(samplePos.y - 0.5f);
+    float cx = x0 + 0.5f, cy = y0 + 0.5f;
     float fx = saturate(samplePos.x - cx), fy = saturate(samplePos.y - cy);
     const float S = 0.5f;
     float w0x = fx * (fx * (-S * fx + 2.0f * S) - S), w0y = fy * (fy * (-S * fy + 2.0f * S) - S);
@@ -74,8 +77,8 @@ __device__ __forceinline__ CatRomSetup SetupCatRom(f2 samplePos, const float* in
     s.u01x *= invSize[0]; s.u01y *= invSize[1]; s.u01z *= invSize[0]; s.u01w *= invSize[1];
     s.u23x *= invSize[0]; s.u23y *= invSize[1]; s.u23z *= invSize[0]; s.u23w *= invSize[1];
     s.u4x *= invSize[0];  s.u4y *= invSize[1];
-    s.bx = (int)cx;
-    s.by = (int)cy;
+    s.bx = (int)x0;
+    s.by = (int)y0;
     s.tcx = tcx;
     s.tcy = tcy;
     s.bicubic = useBicubic;
@@ -118,14 +121,16 @@ __device__ __forceinline__ float ResolveCatRom1(const CatRomSetup& s, const Surf
 }
 // tex.Load(origin + offset) * customWeights, out-of-bounds loads return 0
 __device__ __forceinline__ float LoadOrZero1(const Surf& s, int x, int y) { return Inside(s, x, y) ? LoadR16F(s, x, y) : 0.0f; }
-__device__ __forceinline__ float BilinearCustom1Sum(const CatRomSetup& s, const Surf& tex, f4 cw)
+__device__ __forceinline__ float BilinearCustom1Sum(const Surf& tex, int bx, int by, f4 cw)
 {
-    return LoadOrZero1(tex, s.bx, s.by) * cw.x + LoadOrZero1(tex, s.bx + 1, s.by) * cw.y + LoadOrZero1(tex, s.bx, s.by + 1) * cw.z +
-           LoadOrZero1(tex, s.bx + 1, s.by + 1) * cw.w;
+    return LoadOrZero1(tex, bx, by) * cw.x + LoadOrZero1(tex, bx + 1, by) * cw.y + LoadOrZero1(tex, bx, by + 1) * cw.z + LoadOrZero1(tex, bx + 1, by + 1) * cw.w;
 }
 __device__ __forceinline__ float ResolveBilinearCustom1(const CatRomSetup& s, const Surf& tex, f4 cw)
 {
-    float v = FootprintLocal(tex, s.by, s.by + 1) ? BilinearCustom1Sum(s, Near(tex), cw) : BilinearCustom1Sum(s, tex, cw);
+    // the reference loads these four texels at int2(centerPos), a conversion that rounds towards zero: a footprint that starts
+    // left of or above texel 0 is loaded one texel later than the CatRom footprint (Common.hlsli:648-656)
+    const int bx = s.bx < 0 ? s.bx + 1 : s.bx, by = s.by < 0 ? s.by + 1 : s.by;
+    float v = FootprintLocal(tex, by, by + 1) ? BilinearCustom1Sum(Near(tex), bx, by, cw) : BilinearCustom1Sum(tex, bx, by, cw);
     float sum = cw.x + cw.y + cw.z + cw.w;
     return sum < 0.0001f ? 0.0f : v / sum;
 }

@@ -119,17 +119,15 @@ __global__ void __launch_bounds__(256) SigmaClassifyTilesKernel(const __grid_con
     {
         int idx = i * 32 + lane;
         int x = tx * 16 + (idx & 15), y = ty * 16 + (idx >> 4);
-        float h = 0.0f, z = 0.0f;
+        // every texture reads 0 out of its own bounds: viewZ is read at rectOrigin + pixel (a view that ends earlier under dynamic
+        // resolution), the penumbra and the translucency at the pixel itself
+        const float h = Inside(a.penumbra, x, y) ? LoadR16F(a.penumbra, x, y) : 0.0f;
+        const float z = Inside(a.z, x, y) ? LoadR32F(a.z, x, y) : 0.0f;
         bool isOpaque = true;
-        if (Inside(a.z, x, y))
+        if (TR) // SIGMA_ClassifyTiles.hlsli:45-48: luminance of the translucency colour (out-of-bounds loads read 0: opaque)
         {
-            h = LoadR16F(a.penumbra, x, y);
-            z = LoadR32F(a.z, x, y);
-            if (TR) // SIGMA_ClassifyTiles.hlsli:45-48: luminance of the translucency colour (out-of-bounds loads read 0: opaque)
-            {
-                const f4 t = UnpackRGBA8(LoadU32(a.translucency, x, y));
-                isOpaque = (t.y * 0.2126f + t.z * 0.7152f + t.w * 0.0722f) < 0.003f;
-            }
+            const f4 t = Inside(a.translucency, x, y) ? UnpackRGBA8(LoadU32(a.translucency, x, y)) : mk4(0.0f);
+            isOpaque = (t.y * 0.2126f + t.z * 0.7152f + t.w * 0.0722f) < 0.003f;
         }
         float viewZ = fabsf(z * a.viewZScale);
         bool isInf = viewZ > a.denoisingRange, isShadow = h == 0.0f, isLit = sg::IsLit(h);

@@ -163,23 +163,28 @@ class SideBySide(object):
                 if name.startswith("IN_"):
                     self.ctx.upload(getattr(nrd.ResourceType, name), 0, np.ascontiguousarray(arr))
             for i in range(n):
-                d = nrd.Dispatch(raw[i], pipelines)
-                self._sync_to_gpu(d)
-                floor = self.cpu_alt and self._has_floor(d)
-                if floor:
-                    for alt_den in self.cpu_alt:
-                        for _, rtype, index in d.resources:
-                            alt_den.resolve(rtype, index)[0][...] = self.cpu.resolve(rtype, index)[0]
-                self.ctx.execute_raw(C.byref(raw[i]))
-                self.torch.cuda.synchronize()
-                self._cpu_run(d)
-                if floor:
-                    for alt_den in self.cpu_alt:
-                        alt_den.run_dispatch(d)
-                self._compare_outputs(f, d)
+                self._dispatch(f, raw[i], pipelines)
             if f == 0:
                 self.cpu.set_inputs(fr)  # the frame-0 clears also zero IN_MV (reference quirk), restore it
         return self.report
+
+    def _dispatch(self, f, raw_i, pipelines):
+        """One dispatch on the re-synchronised state: the kernels, the oracle and, for a pass with a noise floor, the perturbed
+        oracle builds on the same inputs; then every texture the pass writes is compared."""
+        d = nrd.Dispatch(raw_i, pipelines)
+        self._sync_to_gpu(d)
+        floor = self.cpu_alt and self._has_floor(d)
+        if floor:
+            for alt_den in self.cpu_alt:
+                for _, rtype, index in d.resources:
+                    alt_den.resolve(rtype, index)[0][...] = self.cpu.resolve(rtype, index)[0]
+        self.ctx.execute_raw(C.byref(raw_i))
+        self.torch.cuda.synchronize()
+        self._cpu_run(d)
+        if floor:
+            for alt_den in self.cpu_alt:
+                alt_den.run_dispatch(d)
+        self._compare_outputs(f, d)
 
     def _run_per_pass_rects(self, frames, rect_fn):
         for f in range(frames):
@@ -195,12 +200,7 @@ class SideBySide(object):
                 if name.startswith("IN_"):
                     self.ctx.upload(getattr(nrd.ResourceType, name), 0, np.ascontiguousarray(arr))
             for i in range(n):
-                d = nrd.Dispatch(raw[i], pipelines)
-                self._sync_to_gpu(d)
-                self.ctx.execute_raw(C.byref(raw[i]))
-                self.torch.cuda.synchronize()
-                self._cpu_run(d)
-                self._compare_outputs(f, d)
+                self._dispatch(f, raw[i], pipelines)
             if f == 0:
                 self.cpu.set_inputs(fr, rect_origin=origin)  # the frame-0 clears also zero IN_MV (reference quirk), restore it
         return self.report

@@ -87,8 +87,9 @@ CASES = {
 
 
 def run_case(name, variant="", size=None):
-    """variant: which build of the oracle (oracle_runner.oracle_lib).  Returns {shader: dict(outputs, min_fraction, min_bytes_equal, worst, changed)} over all dispatches of the case that have a
-    compiled reference shader, and the list of dispatched shaders that have none."""
+    """variant: which build of the oracle (oracle_runner.oracle_lib).  Returns {shader: dict(outputs, min_fraction, min_bytes_equal,
+    min_bytes_equal_after_frame0, worst, changed)} over all dispatches of the case that have a compiled reference shader, and the
+    list of dispatched shaders that have none."""
     den_name, settings_fn, common, frame_fn, frames = CASES[name][:5]
     den = getattr(nrd.Denoiser, den_name)
     W, H = size or (96, 64)
@@ -115,10 +116,13 @@ def run_case(name, variant="", size=None):
                 if den_name == "REBLUR_DIFFUSE" and nrd.Format(fmt) == nrd.Format.R16_UINT:  # (see the module docstring)
                     mine, ref = mine & 0xF03F, ref & 0xF03F
                 frac, worst = orr.compare(mine, ref, fmt, layout=layout)
-                s = stats.setdefault(d.shaderFileName[:-3], dict(outputs=0, min_fraction=1.0, min_bytes_equal=1.0, worst=0.0, changed=0.0))
+                s = stats.setdefault(d.shaderFileName[:-3], dict(outputs=0, min_fraction=1.0, min_bytes_equal=1.0, min_bytes_equal_after_frame0=1.0, worst=0.0, changed=0.0))
                 s["outputs"] += 1
                 s["min_fraction"] = min(s["min_fraction"], frac)
-                s["min_bytes_equal"] = min(s["min_bytes_equal"], float((mine.view(np.uint8) == ref.view(np.uint8)).mean()))
+                equal = float((mine.view(np.uint8) == ref.view(np.uint8)).mean())
+                s["min_bytes_equal"] = min(s["min_bytes_equal"], equal)
+                if f > 0:
+                    s["min_bytes_equal_after_frame0"] = min(s["min_bytes_equal_after_frame0"], equal)
                 s["worst"] = max(s["worst"], worst)
                 s["changed"] = max(s["changed"], float((ref.view(np.uint8) != before.view(np.uint8)).mean()))
         if f == 0:
