@@ -410,7 +410,13 @@ NRD_API nrd::Result nrdCudaConnectPeers(NrdCudaContext* context, uint32_t rank, 
 
 // Enqueues one inter-GPU barrier on `stream` (no-op on one GPU).  nrdCudaDenoise starts with one -- the input strips the
 // peers wrote on their streams are complete before the first pass reads them -- and nrdCudaExecuteDispatch ends with one;
-// applications that walk the dispatch list themselves call this once per frame before the first dispatch.
+// applications that walk the dispatch list themselves call this once per frame before the first dispatch, and AFTER the
+// frame's SetCommonSettings: under dynamic resolution with CommonSettings::rectOrigin[1] != 0 connected strips copy the guide
+// inputs (IN_VIEWZ, IN_NORMAL_ROUGHNESS, IN_MV and the optional inputs the settings switch on) to the rect origin here, followed
+// by a second barrier; a dispatch whose rectOrigin differs from the one seen here returns INVALID_ARGUMENT.
+// Memory: every strip-mode context reserves those copies in its arena at creation -- 23 bytes per texel of
+// resourceWidth x (stripHeight + 2 x haloRows), rows padded to 256 bytes (about 113 MB per rank for two 3840x2160 strips with
+// haloRows 96) -- because the arena is mapped by the peers once.
 NRD_API nrd::Result nrdCudaBarrier(NrdCudaContext* context, void* stream);
 // cudaStreamSynchronize + check that no inter-GPU barrier timed out (a peer that died or fell out of step).
 NRD_API nrd::Result nrdCudaSynchronize(NrdCudaContext* context, void* stream);
@@ -419,7 +425,10 @@ NRD_API nrd::Result nrdCudaSynchronize(NrdCudaContext* context, void* stream);
 // Profiling aid (multi-GPU balance): with timing on, every dispatch of nrdCudaDenoise / nrdCudaExecuteDispatch is bracketed by CUDA
 // events on its stream -- kernelMs[i] = the pass kernel alone, exchangeMs[i] = its ghost-row push + inter-GPU barrier (i.e. the
 // NVLink copy plus the wait for the slowest neighbour).  nrdCudaGetTiming synchronises the events recorded since the last call
-// (at most 64 dispatches are kept) and returns how many there were.
+// (at most 64 dispatches are kept) and returns how many there were.  Frames of connected strips with rectOrigin[1] != 0 add two
+// slots: the first of the frame is the copy of the guide inputs to the rect origin (exchangeMs = the barrier after it), and the
+// slot right after REBLUR temporal stabilization with isBaseColorMetalnessAvailable is the copy of IN_MV back to the
+// application's strip (exchangeMs = 0).  Clear dispatches are not timed.
 NRD_API nrd::Result nrdCudaSetTiming(NrdCudaContext* context, int32_t enable);
 NRD_API nrd::Result nrdCudaGetTiming(NrdCudaContext* context, float* kernelMs, float* exchangeMs, uint32_t capacity, uint32_t* count);
 NRD_API const char* nrdCudaGetLastError(NrdCudaContext* context);

@@ -5,7 +5,14 @@ namespace nrdb200
 {
 cudaError_t LaunchPass(const PassLaunch& p)
 {
-    if (p.rowEnd <= p.rowBegin) return cudaSuccess; // a rank without rows still takes part in the barriers
+    // A rank without rows (a strip below the rect) launches nothing but still takes part in the barriers -- except for the two
+    // passes whose grids do not follow rowBegin / rowEnd, because one GPU writes rows beyond the rect there too:
+    //   ClassifyTiles that builds the guide: the tiles of the rect may cover the rank's ghost rows, which it decodes itself (the
+    //     guide is never pushed);
+    //   SIGMA SmoothTiles: every tile row of the texture, beyond the rect from the clamped tiles of the rect; the bicubic tile
+    //     fetch at the rect's bottom edge reads them.
+    const bool fullGrid = (p.kind.pass == Pass::ClassifyTiles && p.guideMode == 1) || (p.kind.family == Family::SIGMA && p.kind.pass == Pass::SmoothTiles);
+    if (p.rowEnd <= p.rowBegin && !fullGrid) return cudaSuccess;
     if (p.kind.pass == Pass::SplitScreen || p.kind.family == Family::REFERENCE) return LaunchAux(p);
     switch (p.kind.family)
     {
@@ -41,6 +48,7 @@ cudaError_t SetPeerTables(int slot, const PeerTable* table)
     if (e == cudaSuccess) e = SetPeerTableSigma(slot, table);
     if (e == cudaSuccess) e = SetPeerTableRelax(slot, table);
     if (e == cudaSuccess) e = SetPeerTableAux(slot, table);
+    if (e == cudaSuccess) e = SetPeerTableRectOrigin(slot, table);
     return e;
 }
 #endif

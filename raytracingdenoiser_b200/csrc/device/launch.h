@@ -27,7 +27,26 @@ cudaError_t SetPeerTableReblurTemporal(int slot, const PeerTable* table);
 cudaError_t SetPeerTableSigma(int slot, const PeerTable* table);
 cudaError_t SetPeerTableRelax(int slot, const PeerTable* table);
 cudaError_t SetPeerTableAux(int slot, const PeerTable* table);
+cudaError_t SetPeerTableRectOrigin(int slot, const PeerTable* table);
 cudaError_t SetPeerTables(int slot, const PeerTable* table); // all of the above
+
+// Staged guide inputs under rectOrigin.y != 0 (rect_origin.cu): dst texel (x, y) = src texel (x + dx, y + dy) for x in [x0, x1),
+// y in [y0, y1); src is read through the owner lookup, dst rows are held locally.
+struct ShiftedCopy
+{
+    Surf dst, src;
+    int x0, x1, y0, y1;
+    int bytes; // per texel: 1, 4 or 8
+};
+constexpr int kMaxShiftedCopies = 8;
+struct ShiftedCopyArgs
+{
+    ShiftedCopy items[kMaxShiftedCopies];
+    int n, dx, dy;
+};
+// pull = false: GatherRectOriginKernel (frame start), true: PullRectOriginKernel (after a pass wrote a staged input)
+cudaError_t LaunchShiftedCopies(const ShiftedCopyArgs& a, bool pull, cudaStream_t stream);
+cudaError_t PreloadShiftedCopies(); // loads both kernels (see NRD_B200_LAUNCH: nothing may load lazily while a barrier spins)
 #endif
 } // namespace nrdb200
 

@@ -153,6 +153,11 @@ struct NrdCudaContext
     // of every REBLUR frame, read by PrePass / Blur / PostBlur of the same frame
     Texture guide;
     bool guideValid = false;
+    // strip mode: a copy of every guide input (UserTexture::readAtRectOrigin) in the arena, bound instead of the input on frames
+    // that stage (StagesInputs); FrameStart fills it and records for which rectOrigin
+    Texture staged[(size_t)ResourceType::MAX_NUM];
+    bool stagedFrame = false;
+    uint32_t stagedOrigin[2] = {0, 0};
     // roughness table of the REBLUR spatial passes (surf.h PassLaunch::roughnessLut), rebuilt when hitDistanceParameters change
     float* roughnessLut = nullptr;     // device, 1024 x float4 (allocated with the context: no cudaMalloc -- an implicit device
     float* roughnessLutStaging = nullptr; // synchronisation -- may happen while a strip barrier spins); pinned staging copy
@@ -198,6 +203,47 @@ Surf WithRectOrigin(Surf s, ResourceType type, const Texture& t, const CommonSet
     s.lrows -= oy;
     return s;
 }
+
+// Connected strips cannot take that view when rectOrigin.y != 0: shifted by whole rows, a strip's own and ghost rows would hold
+// rows of other strips (the kernels' Near() loads skip the owner lookup).  They stage the guide inputs instead: FrameStart
+// gathers each into a copy with the view's rows in the strip's rows (GatherRectOriginKernel), the passes bind that copy.
+bool StagesInputs(const NrdCudaContext* ctx, const CommonSettings& cs) { return ctx->arena.strip.MultiGpu() && cs.rectOrigin[1] != 0; }
+
+// the guide inputs this frame's passes bind: the optional ones only with their CommonSettings flag (recipes_*.cpp bind a dummy otherwise)
+bool GuideInputRead(ResourceType type, const CommonSettings& cs)
+{
+    switch (type)
+    {
+        case ResourceType::IN_DIFF_CONFIDENCE:
+        case ResourceType::IN_SPEC_CONFIDENCE: return cs.isHistoryConfidenceAvailable;
+        case ResourceType::IN_DISOCCLUSION_THRESHOLD_MIX: return cs.isDisocclusionThresholdMixAvailable;
+        case ResourceType::IN_BASECOLOR_METALNESS: return cs.isBaseColorMetalnessAvailable;
+        default: return true;
+    }
+}
+
+// the staged copy as the passes see it: origin 0, and the size of the one-GPU view, so that every clamp is the same
+Surf StagedView(const NrdCudaContext* ctx, ResourceType type, const CommonSettings& cs)
+{
+    Surf s = ctx->arena.ToSurf(ctx->staged[(uint32_t)type]);
+    s.w -= (int)cs.rectOrigin[0];
+    s.h -= (int)cs.rectOrigin[1];
+    return s;
+}
+
+// the rect must fit the textures the context was created for
+Result CheckRect(NrdCudaContext* ctx, const CommonSettings& cs)
+{
+    const NrdCudaContextDesc& desc = ctx->arena.desc;
+    if (cs.resourceSize[0] != desc.resourceWidth || cs.resourceSize[1] != desc.resourceHeight)
+        return Fail(ctx, Result::INVALID_ARGUMENT, "CommonSettings::resourceSize differs from the size the context was created for");
+    if (cs.rectOrigin[0] + (uint32_t)cs.rectSize[0] > cs.resourceSize[0] || cs.rectOrigin[1] + (uint32_t)cs.rectSize[1] > cs.resourceSize[1])
+        return Fail(ctx, Result::INVALID_ARGUMENT, "rectOrigin + rectSize exceeds resourceSize");
+    return Result::SUCCESS;
+}
+
+// nrdCudaSetTiming: a slot of three events, like a dispatch (before the kernel, after it, after the exchange); nullptr when full / off
+cudaEvent_t* TimingSlot(NrdCudaContext* ctx) { return ctx->timing && ctx->timingCount < 64 ? &ctx->timingEvents[3 * ctx->timingCount++] : nullptr; }
 
 // Roughness table: every function of the 10-bit roughness code alone that the REBLUR spatial filters need, evaluated with the
 // host libm in the reference's operation order (Common.hlsli:311-317 GetSpecMagicCurve, NRD.hlsli:520-523
@@ -285,6 +331,15 @@ NRD_API Result nrdCudaCreateContext(Instance* instance, const NrdCudaContextDesc
         for (Texture& t : *pool) placed.push_back(&t);
     for (Texture& t : ctx->user) placed.push_back(&t);
     placed.push_back(&ctx->guide);
+    // the staged guide inputs (StagesInputs): the arena is mapped by the peers once, so they are carved out of it now, after
+    // everything else
+    if (arena.StripMode())
+        for (const UserTexture& u : kUserTextures)
+            if (u.readAtRectOrigin)
+            {
+                ctx->staged[(uint32_t)u.type] = arena.Describe(u.format, 1, true);
+                placed.push_back(&ctx->staged[(uint32_t)u.type]);
+            }
     if (arena.Allocate(placed.data(), placed.size()) != Result::SUCCESS || cudaMalloc((void**)&ctx->roughnessLut, 1024 * 4 * sizeof(float)) != cudaSuccess ||
         cudaMallocHost((void**)&ctx->roughnessLutStaging, 1024 * 4 * sizeof(float)) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->lutUploaded, cudaEventDisableTiming) != cudaSuccess)
@@ -384,7 +439,10 @@ NRD_API Result nrdCudaGetIpcHandle(NrdCudaContext* ctx, void* handleOut)
 NRD_API Result nrdCudaConnectPeers(NrdCudaContext* ctx, uint32_t rank, uint32_t worldSize, const void* ipcHandles, void* const* arenas, const uint16_t* stripStarts)
 {
     if (!ctx) return Result::INVALID_ARGUMENT;
-    return ctx->arena.ConnectPeers(*ctx->instance, rank, worldSize, ipcHandles, arenas, stripStarts, ctx->lastError);
+    const Result r = ctx->arena.ConnectPeers(*ctx->instance, rank, worldSize, ipcHandles, arenas, stripStarts, ctx->lastError);
+    if (r != Result::SUCCESS || !ctx->arena.strip.MultiGpu()) return r;
+    const cudaError_t e = PreloadShiftedCopies(); // the staging kernels run between barriers too
+    return e == cudaSuccess ? r : Fail(ctx, Result::FAILURE, std::string("loading the staging kernels: ") + cudaGetErrorString(e));
 }
 
 }  // extern "C"
@@ -426,6 +484,33 @@ Result ConvertBound(NrdCudaContext* ctx, const DispatchDesc* d, DescriptorType b
     return Result::SUCCESS;
 }
 
+// After the barrier of a pass that wrote staged guide inputs (REBLUR TemporalStabilization with isBaseColorMetalnessAvailable
+// patches IN_MV at rectOrigin + pixel): every rank copies its own rows of the input back from the staged view, which it reads
+// through the owner lookup, so the application's texture ends the frame as on one GPU.  Texels the pass did not write come back
+// unchanged (the gather copied them there).  No barrier follows: the staged rows are next written by the gather of the next
+// frame, after the frame-start barrier.
+Result PullStaged(NrdCudaContext* ctx, const DispatchDesc* d, const CommonSettings& cs, cudaStream_t stream)
+{
+    const int ox = (int)cs.rectOrigin[0], oy = (int)cs.rectOrigin[1];
+    ShiftedCopyArgs a{};
+    a.dx = -ox;
+    a.dy = -oy;
+    for (uint32_t i = 0; i < d->resourcesNum && a.n < kMaxShiftedCopies; i++)
+    {
+        const ResourceType type = d->resources[i].type;
+        if (d->resources[i].descriptorType != DescriptorType::STORAGE_TEXTURE || !ctx->staged[(uint32_t)type].ptr) continue;
+        const Texture& t = ctx->user[(uint32_t)type];
+        a.items[a.n++] = {ctx->arena.ToSurf(t), ctx->arena.ToSurf(ctx->staged[(uint32_t)type]), ox, (int)t.width, std::max((int)t.firstRow, oy),
+                          (int)t.firstRow + (int)t.rows, (int)BytesPerTexel(t.format)};
+    }
+    if (!a.n) return Result::SUCCESS;
+    cudaEvent_t* ev = TimingSlot(ctx);
+    if (ev) cudaEventRecord(ev[0], stream);
+    const cudaError_t e = LaunchShiftedCopies(a, true, stream);
+    if (ev) cudaEventRecord(ev[1], stream), cudaEventRecord(ev[2], stream);
+    return e == cudaSuccess ? Result::SUCCESS : Fail(ctx, Result::FAILURE, std::string("staged input pull: ") + cudaGetErrorString(e));
+}
+
 // pushMask: bit i set = the ghost rows of resource i must be refreshed after this pass (it is read by a later pass)
 Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream, uint32_t pushMask)
 {
@@ -440,16 +525,16 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     const PassKind kind = ((Scheduler*)ctx->instance)->PipelineKind(d->pipelineIndex);
     const CommonSettings& cs = ((Scheduler*)ctx->instance)->Common();
     // Dynamic resolution (Source/InstanceImpl.cpp:834-856, Shaders/Include/Common.hlsli:200-222): the passes run over rectSize <= resourceSize;
-    // the application's guide inputs are addressed at rectOrigin + pixel (WithRectOrigin), everything else at the pixel itself.
-    if (cs.resourceSize[0] != desc.resourceWidth || cs.resourceSize[1] != desc.resourceHeight)
-        return Fail(ctx, Result::INVALID_ARGUMENT, "CommonSettings::resourceSize differs from the size the context was created for");
-    if (cs.rectOrigin[0] + (uint32_t)cs.rectSize[0] > cs.resourceSize[0] || cs.rectOrigin[1] + (uint32_t)cs.rectSize[1] > cs.resourceSize[1])
-        return Fail(ctx, Result::INVALID_ARGUMENT, "rectOrigin + rectSize exceeds resourceSize");
+    // the application's guide inputs are addressed at rectOrigin + pixel (WithRectOrigin, or their staged copies), everything else at
+    // the pixel itself.
+    const Result rr = CheckRect(ctx, cs);
+    if (rr != Result::SUCCESS) return rr;
     const bool subRect = cs.rectSize[0] != cs.resourceSize[0] || cs.rectSize[1] != cs.resourceSize[1] || cs.rectOrigin[0] || cs.rectOrigin[1];
-    if (subRect && strip.MultiGpu())
-        return Fail(ctx, Result::UNSUPPORTED, "dynamic resolution (rectSize != resourceSize) is not implemented for multi-GPU strips");
     if (ctx->arena.StripMode() && !strip.connected && (desc.stripY0 != 0 || desc.stripY1 != desc.resourceHeight))
         return Fail(ctx, Result::FAILURE, "strip-mode context used before nrdCudaConnectPeers");
+    const bool staged = StagesInputs(ctx, cs);
+    if (staged != ctx->stagedFrame || (staged && (cs.rectOrigin[0] != ctx->stagedOrigin[0] || cs.rectOrigin[1] != ctx->stagedOrigin[1])))
+        return Fail(ctx, Result::INVALID_ARGUMENT, "rectOrigin differs from the one of the frame start: call nrdCudaBarrier after SetCommonSettings (strips stage the guide inputs there)");
 
     PassLaunch p{};
     p.kind = kind;
@@ -465,7 +550,9 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
         const ResourceDesc& r = d->resources[i];
         const Texture* t = Resolve(ctx, r.type, r.indexInPool);
         if (!t) return Fail(ctx, Result::INVALID_ARGUMENT, std::string("unbound resource ") + GetResourceTypeString(r.type) + " for " + d->name);
-        p.tex[i] = WithRectOrigin(ctx->arena.ToSurf(*t), r.type, *t, cs);
+        if (kind.family == Family::CLEAR) p.tex[i] = ctx->arena.ToSurf(*t); // a clear zeroes the whole texture, whatever the rect
+        else if (staged && ctx->staged[(uint32_t)r.type].ptr) p.tex[i] = StagedView(ctx, r.type, cs);
+        else p.tex[i] = WithRectOrigin(ctx->arena.ToSurf(*t), r.type, *t, cs);
         p.texBytes[i] = (uint8_t)BytesPerTexel(t->format);
     }
     // checkerboarded REBLUR inputs (ReblurSettings::checkerboardMode) bind the same passes: the pre-pass resolves them, temporal
@@ -480,7 +567,7 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     {
         const Texture* nr = Resolve(ctx, ResourceType::IN_NORMAL_ROUGHNESS, 0);
         if (!nr) return Fail(ctx, Result::INVALID_ARGUMENT, "unbound resource IN_NORMAL_ROUGHNESS for ClassifyTiles (it also builds the guide surface)");
-        p.guideNr = WithRectOrigin(ctx->arena.ToSurf(*nr), ResourceType::IN_NORMAL_ROUGHNESS, *nr, cs);
+        p.guideNr = staged ? StagedView(ctx, ResourceType::IN_NORMAL_ROUGHNESS, cs) : WithRectOrigin(ctx->arena.ToSurf(*nr), ResourceType::IN_NORMAL_ROUGHNESS, *nr, cs);
         p.guideMode = 1;
     }
     else if (readsGuide)
@@ -526,7 +613,16 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
                               : cudaSuccess;
     }
     else if (isClear)
+    {
         e = LaunchClear(p);
+        // the passes of this frame read the staged copy of a guide input (IN_MV is a storage output): it is zeroed too
+        const Texture* copy = d->resourcesNum ? &ctx->staged[(uint32_t)d->resources[0].type] : nullptr;
+        if (e == cudaSuccess && staged && copy && copy->ptr)
+        {
+            p.tex[0] = ctx->arena.ToSurf(*copy);
+            e = LaunchClear(p);
+        }
+    }
     else
     {
         if (timed) cudaEventRecord(ctx->timingEvents[3 * slot + 0], p.stream);
@@ -541,7 +637,11 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     const Texture* list[33];
     uint32_t n = 0;
     for (uint32_t i = 0; i < d->resourcesNum && !isClear; i++) // clears zero the ghost rows locally
-        if ((pushMask >> i) & 1u) list[n++] = Resolve(ctx, d->resources[i].type, d->resources[i].indexInPool);
+        if ((pushMask >> i) & 1u)
+        {
+            const Texture* copy = &ctx->staged[(uint32_t)d->resources[i].type];
+            list[n++] = staged && copy->ptr ? copy : Resolve(ctx, d->resources[i].type, d->resources[i].indexInPool); // what the pass wrote
+        }
     // (the guide surface needs no push: ClassifyTiles decodes its ghost rows from the ghost rows of the inputs, which arrived with the
     // frame-start push; the barrier below still separates it from the neighbours' far taps, which load the guide from its owner)
     const Result pr = ctx->arena.PushGhostsAndBarrier(list, n, p.stream, ctx->lastError);
@@ -550,7 +650,7 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
         cudaEventRecord(ctx->timingEvents[3 * slot + 2], p.stream);
         ctx->timingCount = slot + 1;
     }
-    return pr;
+    return pr == Result::SUCCESS && staged && !isClear ? PullStaged(ctx, d, cs, p.stream) : pr;
 }
 
 uint32_t StorageMask(const DispatchDesc* d)
@@ -561,14 +661,45 @@ uint32_t StorageMask(const DispatchDesc* d)
     return m;
 }
 
-// frame start: the input strips the application just wrote are pushed to the neighbours' ghost rows, then all ranks meet
+// frame start: the input strips the application just wrote are pushed to the neighbours' ghost rows, then all ranks meet.
+// Frames that stage (StagesInputs, decided from the CommonSettings set last) then gather the guide inputs into their staged
+// copies -- own and ghost rows, straight from the inputs through the owner lookup -- and meet once more before any pass reads them.
 Result FrameStart(NrdCudaContext* ctx, void* stream)
 {
     const Texture* list[std::size(kUserTextures)];
     uint32_t n = 0;
     for (const UserTexture& u : kUserTextures)
         if (u.isInput && ctx->user[(uint32_t)u.type].ptr) list[n++] = &ctx->user[(uint32_t)u.type];
-    return ctx->arena.PushGhostsAndBarrier(list, n, (cudaStream_t)stream, ctx->lastError);
+    Result r = ctx->arena.PushGhostsAndBarrier(list, n, (cudaStream_t)stream, ctx->lastError);
+    const CommonSettings& cs = ((Scheduler*)ctx->instance)->Common();
+    ctx->stagedFrame = false;
+    if (r != Result::SUCCESS || !StagesInputs(ctx, cs)) return r;
+    r = CheckRect(ctx, cs);
+    if (r != Result::SUCCESS) return r;
+    const int ox = (int)cs.rectOrigin[0], oy = (int)cs.rectOrigin[1], W = ctx->arena.desc.resourceWidth, H = ctx->arena.desc.resourceHeight;
+    ShiftedCopyArgs a{};
+    a.dx = ox;
+    a.dy = oy;
+    for (const UserTexture& u : kUserTextures)
+    {
+        const Texture& copy = ctx->staged[(uint32_t)u.type];
+        if (!copy.ptr || !GuideInputRead(u.type, cs) || a.n == kMaxShiftedCopies) continue;
+        const Surf dst = ctx->arena.ToSurf(copy); // the rows held locally that lie in the view, i.e. in [0, H - oy)
+        a.items[a.n++] = {dst, ctx->arena.ToSurf(ctx->user[(uint32_t)u.type]), 0, W - ox, std::max(dst.ly0, 0), std::min(dst.ly0 + (int)dst.lrows, H - oy),
+                          (int)BytesPerTexel(copy.format)};
+    }
+    cudaEvent_t* ev = TimingSlot(ctx);
+    if (ev) cudaEventRecord(ev[0], (cudaStream_t)stream);
+    const cudaError_t e = LaunchShiftedCopies(a, false, (cudaStream_t)stream);
+    if (ev) cudaEventRecord(ev[1], (cudaStream_t)stream);
+    if (e != cudaSuccess) return Fail(ctx, Result::FAILURE, std::string("staged input gather: ") + cudaGetErrorString(e));
+    r = ctx->arena.PushGhostsAndBarrier(nullptr, 0, (cudaStream_t)stream, ctx->lastError); // the peers' far taps read these rows
+    if (ev) cudaEventRecord(ev[2], (cudaStream_t)stream);
+    if (r != Result::SUCCESS) return r;
+    ctx->stagedFrame = true;
+    ctx->stagedOrigin[0] = (uint32_t)ox;
+    ctx->stagedOrigin[1] = (uint32_t)oy;
+    return r;
 }
 } // namespace
 
