@@ -418,6 +418,22 @@ NRD_API nrd::Result nrdCudaConnectPeers(NrdCudaContext* context, uint32_t rank, 
 // resourceWidth x (stripHeight + 2 x haloRows), rows padded to 256 bytes (about 113 MB per rank for two 3840x2160 strips with
 // haloRows 96) -- because the arena is mapped by the peers once.
 NRD_API nrd::Result nrdCudaBarrier(NrdCudaContext* context, void* stream);
+// Collective: every connected rank calls it with the same table, between two frames -- after the last nrdCudaExecuteDispatch or
+// nrdCudaDenoise of a frame and before the next frame's SetCommonSettings / nrdCudaBarrier.  Moves the strip boundaries: `stripStarts`
+// follows the rules of nrdCudaConnectPeers (worldSize + 1 entries, the first 0 and the last the frame height; every strip starts on
+// a multiple of 16, owns rows, at most stripHeight of them, and every strip but the last holds at least haloRows).  Every texture
+// of the context -- histories, transient textures, the IN_* / OUT_* strips -- keeps its contents: its rows move to their new
+// owners, so the next frame continues accumulation and computes the same bits as without the move.  Enqueued on `stream` with no
+// host synchronisation (three inter-GPU barriers, one copy kernel, one copy back); the stripY0 / stripY1 of the context change with
+// it.  Afterwards the application writes the next frame's IN_* rows, and reads OUT_* rows, through nrdCudaGetTexture /
+// nrdCudaCopyTexture with the new firstRow / rowsNum; a dispatch before the next frame start returns FAILURE.
+// The library does not choose cuts: see strips.StripDenoiser for a policy.  A larger stripHeight at creation is what makes uneven
+// cuts possible, and the arena grows in proportion to it.  Memory: a scratch buffer the size of the arena, allocated and freed
+// on `stream` (cudaMallocAsync), exists only while the call runs.
+// INVALID_ARGUMENT: null context or table, or a table that breaks the rules -- refused before anything is enqueued, alike on every
+// rank.  UNSUPPORTED: a one-GPU context, or a strip context that is not connected.  FAILURE: an earlier barrier of the context
+// timed out.  A connected world of one accepts the identity table only, and does nothing.
+NRD_API nrd::Result nrdCudaRepartition(NrdCudaContext* context, const uint16_t* stripStarts, void* stream);
 // cudaStreamSynchronize + check that no inter-GPU barrier timed out (a peer that died or fell out of step).
 NRD_API nrd::Result nrdCudaSynchronize(NrdCudaContext* context, void* stream);
 

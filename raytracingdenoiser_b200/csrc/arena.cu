@@ -71,6 +71,44 @@ struct PushArgs
 {
     PushItem items[kMaxPushItems];
 };
+
+// rows [firstRow, firstRow + rows) of t belong to the strip [y0, y1) (full-resolution rows)
+void SetRows(Texture& t, uint32_t y0, uint32_t y1)
+{
+    int first = (int)y0 / t.downsample, last = ((int)y1 + t.downsample - 1) / t.downsample;
+    if (last > (int)t.height) last = t.height;
+    if (first > last) first = last;
+    t.firstRow = (uint16_t)first;
+    t.rows = (uint16_t)(last - first);
+}
+
+PeerTable MakePeerTable(const long long* peerDelta, const uint32_t* stripStart, uint32_t worldSize)
+{
+    PeerTable table{};
+    for (uint32_t i = 0; i < (uint32_t)kMaxPeers; i++) table.delta[i] = peerDelta[i];
+    for (uint32_t i = 0; i <= (uint32_t)kMaxPeers; i++) table.start[i] = i <= worldSize ? (int)stripStart[i] : 0x7fffffff;
+    if (worldSize < (uint32_t)kMaxPeers) table.start[worldSize] = 0x7fffffff; // rows >= start[world] do not exist: never counted as an owner change
+    return table;
+}
+
+// One owned texture of the repartition: where it lies in the texture region of every arena, and its rows under the new table.
+struct MigrateItem
+{
+    unsigned long long offset; // from the start of the texture region (arena + kArenaHeader)
+    unsigned pitch;            // a multiple of 256
+    uint16_t height, allocRows, haloRows, downsample;
+    uint16_t firstRow, rows;   // new
+};
+constexpr int kMaxMigrateItems = 128;
+struct MigrateArgs
+{
+    const uint8_t* textures; // local texture region; a peer's is at + old.delta[peer]
+    uint8_t* scratch;        // a copy of the texture region laid out like it, then the new table
+    PeerTable* tableOut;
+    PeerTable old, next;     // the strip tables before and after (the kernel must not read g_peerTable: it is switched later)
+    unsigned n;
+    MigrateItem items[kMaxMigrateItems];
+};
 } // namespace
 
 namespace nrdb200
@@ -156,6 +194,33 @@ __global__ void __launch_bounds__(256) GhostPushKernel(const __grid_constant__ P
     if (last) StripBarrierBody(b, threadIdx.x);
 }
 
+// Repartition: texture blockIdx.y, local rows blockIdx.x, +gridDim.x, ... of its new layout.  A row of the new window (own rows and
+// ghost rows inside the frame) is copied from the rank that owns it under the old table, where it is an own row; every other row
+// (beyond the frame, or the unused tail of a strip shorter than the reserved height) is zeroed.  Rows are whole pitched rows,
+// multiples of 256 B: 16-byte vectors whatever the format.  Downsampled textures count rows in their own units, as PeerRow does.
+__global__ void __launch_bounds__(256) MigrateRowsKernel(const __grid_constant__ MigrateArgs a)
+{
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *a.tableOut = a.next;
+    const MigrateItem& it = a.items[blockIdx.y];
+    const unsigned n16 = it.pitch / 16;
+    const int window = (int)it.rows + 2 * (int)it.haloRows; // the rows kept current (Arena::ToSurf lrows)
+    for (int k = blockIdx.x; k < (int)it.allocRows; k += gridDim.x)
+    {
+        const int y = (int)it.firstRow - (int)it.haloRows + k;
+        const uint4* src = nullptr;
+        if (k < window && y >= 0 && y < (int)it.height)
+        {
+            const int yFull = y * (int)it.downsample;
+            int owner = 0;
+#pragma unroll
+            for (int j = 1; j < kMaxPeers; j++) owner += yFull >= a.old.start[j] ? 1 : 0;
+            src = (const uint4*)(a.textures + a.old.delta[owner] + it.offset + (size_t)(y - a.old.start[owner] / (int)it.downsample + (int)it.haloRows) * it.pitch);
+        }
+        uint4* dst = (uint4*)(a.scratch + it.offset + (size_t)k * it.pitch);
+        for (unsigned c = threadIdx.x; c < n16; c += blockDim.x) dst[c] = src ? src[c] : make_uint4(0, 0, 0, 0);
+    }
+}
+
 uint32_t BytesPerTexel(Format f)
 {
 #define NRD_B200_BPT(name, bytes, isInt) bytes,
@@ -171,12 +236,7 @@ Texture Arena::Describe(Format format, uint16_t downsample, bool owned, void* pt
     t.downsample = downsample;
     t.width = uint16_t((desc.resourceWidth + downsample - 1) / downsample);
     t.height = uint16_t((desc.resourceHeight + downsample - 1) / downsample);
-    // rows [firstRow, firstRow + rows) belong to the context
-    int first = desc.stripY0 / downsample, last = (desc.stripY1 + downsample - 1) / downsample;
-    if (last > (int)t.height) last = t.height;
-    if (first > last) first = last;
-    t.firstRow = (uint16_t)first;
-    t.rows = (uint16_t)(last - first);
+    SetRows(t, desc.stripY0, desc.stripY1);
     t.haloRows = uint16_t(strip.halo / downsample);
     t.allocRows = owned && StripMode() ? uint16_t(desc.stripHeight / downsample + 2 * t.haloRows) : t.rows;
     t.owned = owned;
@@ -266,14 +326,8 @@ Result Arena::ConnectPeers(const Instance& instance, uint32_t rank, uint32_t wor
         if (!stripStarts && (i == worldSize || y > desc.resourceHeight)) y = desc.resourceHeight;
         s.stripStart[i] = y;
     }
-    if (s.stripStart[0] != 0 || s.stripStart[worldSize] != desc.resourceHeight) return Fail(error, Result::INVALID_ARGUMENT, "the strips do not cover the frame");
-    for (uint32_t i = 0; i < worldSize; i++)
-    {
-        const uint32_t rows = s.stripStart[i + 1] - s.stripStart[i];
-        if (s.stripStart[i + 1] <= s.stripStart[i] || s.stripStart[i] % 16 != 0 || rows > desc.stripHeight)
-            return Fail(error, Result::INVALID_ARGUMENT, "every strip must start on a multiple of 16, own rows and fit stripHeight");
-        if (rows < s.halo && i + 1 < worldSize) return Fail(error, Result::INVALID_ARGUMENT, "haloRows exceeds the height of a strip (ghost rows are refreshed by the direct neighbours only)");
-    }
+    const Result pr = CheckPartition(s.stripStart, worldSize, error);
+    if (pr != Result::SUCCESS) return pr;
     if (s.stripStart[rank] != desc.stripY0 || s.stripStart[rank + 1] != desc.stripY1) return Fail(error, Result::INVALID_ARGUMENT, "stripY0/stripY1 do not match the strip table");
     cudaSetDevice(desc.device);
     for (uint32_t i = 0; i < worldSize; i++)
@@ -296,10 +350,7 @@ Result Arena::ConnectPeers(const Instance& instance, uint32_t rank, uint32_t wor
             if (!g_slotUsed[k]) { g_slotUsed[k] = true; s.peerSlot = k; }
     }
     if (s.peerSlot < 0) return Fail(error, Result::FAILURE, "too many strip-mode contexts in one process");
-    PeerTable table{};
-    for (uint32_t i = 0; i < (uint32_t)kMaxPeers; i++) table.delta[i] = s.peerDelta[i];
-    for (uint32_t i = 0; i <= (uint32_t)kMaxPeers; i++) table.start[i] = i <= worldSize ? (int)s.stripStart[i] : 0x7fffffff;
-    if (worldSize < (uint32_t)kMaxPeers) table.start[worldSize] = 0x7fffffff; // rows >= start[world] do not exist: never counted as an owner change
+    const PeerTable table = MakePeerTable(s.peerDelta, s.stripStart, worldSize);
     cudaError_t e = SetPeerTables(s.peerSlot, &table);
     if (e != cudaSuccess) return Fail(error, Result::FAILURE, std::string("peer table: ") + cudaGetErrorString(e));
     s.rank = rank;
@@ -313,7 +364,87 @@ Result Arena::ConnectPeers(const Instance& instance, uint32_t rank, uint32_t wor
     (void)cudaFuncGetAttributes(&fa, ClearKernel);
     (void)cudaFuncGetAttributes(&fa, StripBarrierKernel);
     (void)cudaFuncGetAttributes(&fa, GhostPushKernel);
+    (void)cudaFuncGetAttributes(&fa, MigrateRowsKernel);
     return Result::SUCCESS;
+}
+
+Result Arena::CheckPartition(const uint32_t* starts, uint32_t worldSize, std::string& error) const
+{
+    if (starts[0] != 0 || starts[worldSize] != desc.resourceHeight) return Fail(error, Result::INVALID_ARGUMENT, "the strips do not cover the frame");
+    for (uint32_t i = 0; i < worldSize; i++)
+    {
+        const uint32_t rows = starts[i + 1] - starts[i];
+        if (starts[i + 1] <= starts[i] || starts[i] % 16 != 0 || rows > desc.stripHeight)
+            return Fail(error, Result::INVALID_ARGUMENT, "every strip must start on a multiple of 16, own rows and fit stripHeight");
+        if (rows < strip.halo && i + 1 < worldSize) return Fail(error, Result::INVALID_ARGUMENT, "haloRows exceeds the height of a strip (ghost rows are refreshed by the direct neighbours only)");
+    }
+    return Result::SUCCESS;
+}
+
+// Order on `stream`, the same on every rank:
+//   barrier A   the previous frame's writes of every rank are complete and visible
+//   MigrateRowsKernel   every row the new partition holds here (own and ghost rows), read from its owner under the OLD table,
+//               into a scratch copy of the texture region; rows outside the frame and the unused tail of a strip read 0
+//   barrier B   no rank still reads the old layout
+//   copy back, scratch -> arena; the new table into every kernel translation unit (stream-ordered: the kernels queued before
+//               still read the old one); the scratch is freed
+//   barrier C   no peer pushes ghost rows (the next frame start) into rows the copy-back still writes
+// Every allocation and copy is stream-ordered: in one process, ranks are contexts of one GPU, and a host call that waits for the
+// device would wait for a barrier spinning for a rank the host has not reached yet.
+Result Arena::Repartition(Texture* const* textures, size_t n, const uint16_t* stripStarts, cudaStream_t stream, std::string& error)
+{
+    if (!StripMode() || !strip.connected) return Fail(error, Result::UNSUPPORTED, "not a connected strip-mode context");
+    if (strip.hostError && *(volatile unsigned*)strip.hostError)
+        return Fail(error, Result::FAILURE, "a strip barrier of this context timed out waiting for a peer (epoch " + std::to_string(*(volatile unsigned*)strip.hostError) + ")");
+    StripState& s = strip;
+    uint32_t starts[kMaxPeers + 1] = {};
+    for (uint32_t i = 0; i <= s.world; i++) starts[i] = stripStarts[i];
+    const Result pr = CheckPartition(starts, s.world, error);
+    if (pr != Result::SUCCESS || !s.MultiGpu()) return pr; // a world of one: the identity table is the only valid one
+    MigrateArgs a{};
+    a.textures = base + kArenaHeader;
+    a.old = MakePeerTable(s.peerDelta, s.stripStart, s.world);
+    a.next = MakePeerTable(s.peerDelta, starts, s.world);
+    uint32_t maxRows = 0;
+    for (size_t i = 0; i < n; i++)
+    {
+        const Texture& t = *textures[i];
+        if (!t.owned) continue;
+        if (a.n == (uint32_t)kMaxMigrateItems) return Fail(error, Result::FAILURE, "repartition: more textures than one launch carries (" + std::to_string(kMaxMigrateItems) + ")");
+        Texture moved = t;
+        SetRows(moved, starts[s.rank], starts[s.rank + 1]);
+        a.items[a.n++] = {(unsigned long long)((uint8_t*)t.ptr - a.textures), (unsigned)t.pitch, t.height, t.allocRows, t.haloRows, t.downsample, moved.firstRow, moved.rows};
+        if (t.allocRows > maxRows) maxRows = t.allocRows;
+    }
+    const size_t region = bytes - kArenaHeader; // every owned texture, in arena order (256-B multiples)
+    // (the pool of the stream's device: the caller's current device, as for every other call of the executor)
+    cudaError_t e = cudaMallocAsync((void**)&a.scratch, region + sizeof(PeerTable), stream);
+    if (e != cudaSuccess) return Fail(error, Result::FAILURE, std::string("repartition scratch: ") + cudaGetErrorString(e));
+    a.tableOut = (PeerTable*)(a.scratch + region);
+    Result r = PushGhostsAndBarrier(nullptr, 0, stream, error); // A
+    if (r == Result::SUCCESS)
+    {
+        MigrateRowsKernel<<<dim3(maxRows < 256u ? maxRows : 256u, a.n), 256, 0, stream>>>(a);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) r = Fail(error, Result::FAILURE, std::string("repartition: ") + cudaGetErrorString(e));
+    }
+    if (r == Result::SUCCESS) r = PushGhostsAndBarrier(nullptr, 0, stream, error); // B
+    if (r == Result::SUCCESS)
+    {
+        e = cudaMemcpyAsync(base + kArenaHeader, a.scratch, region, cudaMemcpyDeviceToDevice, stream);
+        if (e == cudaSuccess) e = SetPeerTables(s.peerSlot, a.tableOut, &stream);
+        if (e != cudaSuccess) r = Fail(error, Result::FAILURE, std::string("repartition: ") + cudaGetErrorString(e));
+    }
+    e = cudaFreeAsync(a.scratch, stream);
+    if (r != Result::SUCCESS) return r;
+    if (e != cudaSuccess) return Fail(error, Result::FAILURE, std::string("repartition: ") + cudaGetErrorString(e));
+    // the host side of the new table: what every later launch, push and nrdCudaGetTexture sees
+    for (uint32_t i = 0; i <= s.world; i++) s.stripStart[i] = starts[i];
+    desc.stripY0 = (uint16_t)starts[s.rank];
+    desc.stripY1 = (uint16_t)starts[s.rank + 1];
+    for (size_t i = 0; i < n; i++)
+        if (textures[i]->owned) SetRows(*textures[i], desc.stripY0, desc.stripY1);
+    return PushGhostsAndBarrier(nullptr, 0, stream, error); // C
 }
 
 Result Arena::PushGhostsAndBarrier(const Texture* const* textures, uint32_t n, cudaStream_t stream, std::string& error)

@@ -4,7 +4,8 @@
 // is a strip of `stripHeight` rows plus ghost rows; arenas are exchanged with CUDA IPC and the kernels read foreign rows straight
 // from the owner (device/common.cuh TexelPtr).  After every pass each rank pushes the rows it wrote next to its neighbours into
 // their ghost rows, signals all its peers and waits for all of them: a pass may read what any rank wrote in the previous pass and
-// may overwrite what any rank read in it.
+// may overwrite what any rank read in it.  The strip table can change between frames (Repartition): every texture keeps its place
+// in the arena, only the rows it holds change.
 #pragma once
 #include "../../include/nrd_b200.h"
 #include "device/surf.h"
@@ -62,6 +63,11 @@ struct Arena
     void Release();
     nrd::Result ConnectPeers(const nrd::Instance& instance, uint32_t rank, uint32_t worldSize, const void* ipcHandles, void* const* arenas,
                              const uint16_t* stripStarts, std::string& error);
+    // the rules of a strip table (worldSize + 1 first rows, the last = frame height) shared by ConnectPeers and Repartition
+    nrd::Result CheckPartition(const uint32_t* starts, uint32_t worldSize, std::string& error) const;
+    // Collective (nrdCudaRepartition): moves the rows of every owned texture in `textures` to their owners under the strip table
+    // `stripStarts` (strip.world + 1 entries) and switches to it.  Enqueued on `stream` without a host synchronisation.
+    nrd::Result Repartition(Texture* const* textures, size_t n, const uint16_t* stripStarts, cudaStream_t stream, std::string& error);
     // MultiGpu(): pushes the boundary rows of `textures`, just written by this rank, to the neighbours, then meets all ranks
     nrd::Result PushGhostsAndBarrier(const Texture* const* textures, uint32_t n, cudaStream_t stream, std::string& error);
     nrd::Result CheckBarriers(std::string& error) const; // fails if a barrier timed out

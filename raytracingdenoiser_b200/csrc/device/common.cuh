@@ -63,9 +63,13 @@ struct Bindings
 #if !defined(NRD_B200_NO_STRIPS)
 // strip geometry, one table per context slot (surf.h)
 static __constant__ PeerTable g_peerTable[kMaxPeerSlots];
-static inline cudaError_t SetPeerTableThisTU(int slot, const PeerTable* table)
+// stream == nullptr: `table` is host memory, copied before the call returns (nrdCudaConnectPeers); else `table` is device memory,
+// copied in order on *stream (nrdCudaRepartition: the kernels queued before the copy still read the old table)
+static inline cudaError_t SetPeerTableThisTU(int slot, const PeerTable* table, const cudaStream_t* stream)
 {
-    return cudaMemcpyToSymbol(g_peerTable, table, sizeof(PeerTable), sizeof(PeerTable) * (size_t)slot);
+    const size_t offset = sizeof(PeerTable) * (size_t)slot;
+    return stream ? cudaMemcpyToSymbolAsync(g_peerTable, table, sizeof(PeerTable), offset, cudaMemcpyDeviceToDevice, *stream)
+                  : cudaMemcpyToSymbol(g_peerTable, table, sizeof(PeerTable), offset);
 }
 // rare path: the row is beyond the ghost rows, fetch it from its owner (callers clamp y to [0, h))
 // (inlined on purpose: a real call gives the kernels a stack frame, and the first launch of a kernel that needs a bigger

@@ -40,15 +40,15 @@ cudaError_t LaunchPass(const PassLaunch& p)
 }
 
 #if !defined(NRD_B200_NO_STRIPS)
-cudaError_t SetPeerTables(int slot, const PeerTable* table)
+cudaError_t SetPeerTables(int slot, const PeerTable* table, const cudaStream_t* stream)
 {
-    cudaError_t e = SetPeerTableReblurSpatial(slot, table);
-    if (e == cudaSuccess) e = SetPeerTableReblurHitDist(slot, table);
-    if (e == cudaSuccess) e = SetPeerTableReblurTemporal(slot, table);
-    if (e == cudaSuccess) e = SetPeerTableSigma(slot, table);
-    if (e == cudaSuccess) e = SetPeerTableRelax(slot, table);
-    if (e == cudaSuccess) e = SetPeerTableAux(slot, table);
-    if (e == cudaSuccess) e = SetPeerTableRectOrigin(slot, table);
+    cudaError_t e = SetPeerTableReblurSpatial(slot, table, stream);
+    if (e == cudaSuccess) e = SetPeerTableReblurHitDist(slot, table, stream);
+    if (e == cudaSuccess) e = SetPeerTableReblurTemporal(slot, table, stream);
+    if (e == cudaSuccess) e = SetPeerTableSigma(slot, table, stream);
+    if (e == cudaSuccess) e = SetPeerTableRelax(slot, table, stream);
+    if (e == cudaSuccess) e = SetPeerTableAux(slot, table, stream);
+    if (e == cudaSuccess) e = SetPeerTableRectOrigin(slot, table, stream);
     return e;
 }
 #endif

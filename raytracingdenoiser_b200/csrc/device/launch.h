@@ -20,15 +20,16 @@ cudaError_t LaunchAux(const PassLaunch& p); // split-screen passes, REFERENCE de
 cudaError_t LaunchPass(const PassLaunch& p); // cudaErrorNotSupported: the pass has no kernel
 
 #if !defined(NRD_B200_NO_STRIPS)
-// peer address table of one context slot, replicated into the constant memory of every kernel translation unit
-cudaError_t SetPeerTableReblurSpatial(int slot, const PeerTable* table);
-cudaError_t SetPeerTableReblurHitDist(int slot, const PeerTable* table);
-cudaError_t SetPeerTableReblurTemporal(int slot, const PeerTable* table);
-cudaError_t SetPeerTableSigma(int slot, const PeerTable* table);
-cudaError_t SetPeerTableRelax(int slot, const PeerTable* table);
-cudaError_t SetPeerTableAux(int slot, const PeerTable* table);
-cudaError_t SetPeerTableRectOrigin(int slot, const PeerTable* table);
-cudaError_t SetPeerTables(int slot, const PeerTable* table); // all of the above
+// peer address table of one context slot, replicated into the constant memory of every kernel translation unit.
+// stream == nullptr: a host table, copied synchronously; else a device table, copied in order on *stream (common.cuh)
+cudaError_t SetPeerTableReblurSpatial(int slot, const PeerTable* table, const cudaStream_t* stream);
+cudaError_t SetPeerTableReblurHitDist(int slot, const PeerTable* table, const cudaStream_t* stream);
+cudaError_t SetPeerTableReblurTemporal(int slot, const PeerTable* table, const cudaStream_t* stream);
+cudaError_t SetPeerTableSigma(int slot, const PeerTable* table, const cudaStream_t* stream);
+cudaError_t SetPeerTableRelax(int slot, const PeerTable* table, const cudaStream_t* stream);
+cudaError_t SetPeerTableAux(int slot, const PeerTable* table, const cudaStream_t* stream);
+cudaError_t SetPeerTableRectOrigin(int slot, const PeerTable* table, const cudaStream_t* stream);
+cudaError_t SetPeerTables(int slot, const PeerTable* table, const cudaStream_t* stream = nullptr); // all of the above
 
 // Staged guide inputs under rectOrigin.y != 0 (rect_origin.cu): dst texel (x, y) = src texel (x + dx, y + dy) for x in [x0, x1),
 // y in [y0, y1); src is read through the owner lookup, dst rows are held locally.

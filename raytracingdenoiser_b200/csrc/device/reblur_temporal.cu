@@ -1384,6 +1384,6 @@ cudaError_t LaunchReblurTemporalStabilization(const PassLaunch& p)
 }
 
 #if !defined(NRD_B200_NO_STRIPS)
-cudaError_t SetPeerTableReblurTemporal(int slot, const PeerTable* table) { return SetPeerTableThisTU(slot, table); }
+cudaError_t SetPeerTableReblurTemporal(int slot, const PeerTable* table, const cudaStream_t* stream) { return SetPeerTableThisTU(slot, table, stream); }
 #endif
 } // namespace nrdb200

@@ -55,6 +55,6 @@ cudaError_t PreloadShiftedCopies()
     return e == cudaSuccess ? cudaFuncGetAttributes(&fa, PullRectOriginKernel) : e;
 }
 
-cudaError_t SetPeerTableRectOrigin(int slot, const PeerTable* table) { return SetPeerTableThisTU(slot, table); }
+cudaError_t SetPeerTableRectOrigin(int slot, const PeerTable* table, const cudaStream_t* stream) { return SetPeerTableThisTU(slot, table, stream); }
 } // namespace nrdb200
 #endif

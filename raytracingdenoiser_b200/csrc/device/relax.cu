@@ -1706,6 +1706,6 @@ cudaError_t LaunchRelax(const PassLaunch& p)
 }
 
 #if !defined(NRD_B200_NO_STRIPS)
-cudaError_t SetPeerTableRelax(int slot, const PeerTable* table) { return SetPeerTableThisTU(slot, table); }
+cudaError_t SetPeerTableRelax(int slot, const PeerTable* table, const cudaStream_t* stream) { return SetPeerTableThisTU(slot, table, stream); }
 #endif
 } // namespace nrdb200

@@ -573,6 +573,6 @@ cudaError_t LaunchSigma(const PassLaunch& p)
 }
 
 #if !defined(NRD_B200_NO_STRIPS)
-cudaError_t SetPeerTableSigma(int slot, const PeerTable* table) { return SetPeerTableThisTU(slot, table); }
+cudaError_t SetPeerTableSigma(int slot, const PeerTable* table, const cudaStream_t* stream) { return SetPeerTableThisTU(slot, table, stream); }
 #endif
 } // namespace nrdb200

@@ -158,6 +158,7 @@ struct NrdCudaContext
     Texture staged[(size_t)ResourceType::MAX_NUM];
     bool stagedFrame = false;
     uint32_t stagedOrigin[2] = {0, 0};
+    bool repartitioned = false; // nrdCudaRepartition ran since the last frame start: no dispatch before the next one
     // roughness table of the REBLUR spatial passes (surf.h PassLaunch::roughnessLut), rebuilt when hitDistanceParameters change
     float* roughnessLut = nullptr;     // device, 1024 x float4 (allocated with the context: no cudaMalloc -- an implicit device
     float* roughnessLutStaging = nullptr; // synchronisation -- may happen while a strip barrier spins); pinned staging copy
@@ -240,6 +241,21 @@ Result CheckRect(NrdCudaContext* ctx, const CommonSettings& cs)
     if (cs.rectOrigin[0] + (uint32_t)cs.rectSize[0] > cs.resourceSize[0] || cs.rectOrigin[1] + (uint32_t)cs.rectSize[1] > cs.resourceSize[1])
         return Fail(ctx, Result::INVALID_ARGUMENT, "rectOrigin + rectSize exceeds resourceSize");
     return Result::SUCCESS;
+}
+
+// every texture the arena holds, in placement order: one arena, identical layout on every rank
+std::vector<Texture*> ArenaTextures(NrdCudaContext* ctx)
+{
+    std::vector<Texture*> placed;
+    for (std::vector<Texture>* pool : {&ctx->permanent, &ctx->transient})
+        for (Texture& t : *pool) placed.push_back(&t);
+    for (Texture& t : ctx->user) placed.push_back(&t);
+    placed.push_back(&ctx->guide);
+    // the staged guide inputs (StagesInputs): the arena is mapped by the peers once, so they are carved out of it too, after
+    // everything else
+    for (const UserTexture& u : kUserTextures)
+        if (ctx->staged[(uint32_t)u.type].owned) placed.push_back(&ctx->staged[(uint32_t)u.type]);
+    return placed;
 }
 
 // nrdCudaSetTiming: a slot of three events, like a dispatch (before the kernel, after it, after the exchange); nullptr when full / off
@@ -326,20 +342,10 @@ NRD_API Result nrdCudaCreateContext(Instance* instance, const NrdCudaContextDesc
     if (arena.StripMode())
         for (const UserTexture& u : kUserTextures) ctx->user[(uint32_t)u.type] = arena.Describe(FindUserTexture(u.type, Translucent(instance))->format, 1, true);
     ctx->guide = arena.Describe(Format::RGBA32_SFLOAT, 1, true);
-    std::vector<Texture*> placed; // one arena, identical layout on every rank
-    for (std::vector<Texture>* pool : {&ctx->permanent, &ctx->transient})
-        for (Texture& t : *pool) placed.push_back(&t);
-    for (Texture& t : ctx->user) placed.push_back(&t);
-    placed.push_back(&ctx->guide);
-    // the staged guide inputs (StagesInputs): the arena is mapped by the peers once, so they are carved out of it now, after
-    // everything else
     if (arena.StripMode())
         for (const UserTexture& u : kUserTextures)
-            if (u.readAtRectOrigin)
-            {
-                ctx->staged[(uint32_t)u.type] = arena.Describe(u.format, 1, true);
-                placed.push_back(&ctx->staged[(uint32_t)u.type]);
-            }
+            if (u.readAtRectOrigin) ctx->staged[(uint32_t)u.type] = arena.Describe(u.format, 1, true);
+    const std::vector<Texture*> placed = ArenaTextures(ctx);
     if (arena.Allocate(placed.data(), placed.size()) != Result::SUCCESS || cudaMalloc((void**)&ctx->roughnessLut, 1024 * 4 * sizeof(float)) != cudaSuccess ||
         cudaMallocHost((void**)&ctx->roughnessLutStaging, 1024 * 4 * sizeof(float)) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->lutUploaded, cudaEventDisableTiming) != cudaSuccess)
@@ -532,6 +538,8 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     const bool subRect = cs.rectSize[0] != cs.resourceSize[0] || cs.rectSize[1] != cs.resourceSize[1] || cs.rectOrigin[0] || cs.rectOrigin[1];
     if (ctx->arena.StripMode() && !strip.connected && (desc.stripY0 != 0 || desc.stripY1 != desc.resourceHeight))
         return Fail(ctx, Result::FAILURE, "strip-mode context used before nrdCudaConnectPeers");
+    if (ctx->repartitioned)
+        return Fail(ctx, Result::FAILURE, "dispatched after nrdCudaRepartition without a frame start: call nrdCudaBarrier (or nrdCudaDenoise) first");
     const bool staged = StagesInputs(ctx, cs);
     if (staged != ctx->stagedFrame || (staged && (cs.rectOrigin[0] != ctx->stagedOrigin[0] || cs.rectOrigin[1] != ctx->stagedOrigin[1])))
         return Fail(ctx, Result::INVALID_ARGUMENT, "rectOrigin differs from the one of the frame start: call nrdCudaBarrier after SetCommonSettings (strips stage the guide inputs there)");
@@ -673,6 +681,7 @@ Result FrameStart(NrdCudaContext* ctx, void* stream)
     Result r = ctx->arena.PushGhostsAndBarrier(list, n, (cudaStream_t)stream, ctx->lastError);
     const CommonSettings& cs = ((Scheduler*)ctx->instance)->Common();
     ctx->stagedFrame = false;
+    ctx->repartitioned = false;
     if (r != Result::SUCCESS || !StagesInputs(ctx, cs)) return r;
     r = CheckRect(ctx, cs);
     if (r != Result::SUCCESS) return r;
@@ -772,6 +781,23 @@ NRD_API Result nrdCudaBarrier(NrdCudaContext* ctx, void* stream)
 {
     if (!ctx) return Result::INVALID_ARGUMENT;
     return FrameStart(ctx, stream);
+}
+
+NRD_API Result nrdCudaRepartition(NrdCudaContext* ctx, const uint16_t* stripStarts, void* stream)
+{
+    if (!ctx) return Result::INVALID_ARGUMENT;
+    if (!stripStarts) return Fail(ctx, Result::INVALID_ARGUMENT, "stripStarts is null");
+    const std::vector<Texture*> textures = ArenaTextures(ctx);
+    const Result r = ctx->arena.Repartition(textures.data(), textures.size(), stripStarts, (cudaStream_t)stream, ctx->lastError);
+    if (r == Result::SUCCESS && ctx->arena.strip.MultiGpu())
+    {
+        // the per-frame state ends with the frame: the next dispatch needs a frame start (input push, staging) under the new table
+        ctx->guideValid = false;
+        ctx->stagedFrame = false;
+        ctx->stagedOrigin[0] = ctx->stagedOrigin[1] = 0;
+        ctx->repartitioned = true;
+    }
+    return r;
 }
 
 NRD_API Result nrdCudaSynchronize(NrdCudaContext* ctx, void* stream)

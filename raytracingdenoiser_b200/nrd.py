@@ -242,6 +242,8 @@ _lib.nrdCudaConnectPeers.argtypes = [C.c_void_p, u32, u32, C.c_void_p, C.POINTER
 _lib.nrdCudaConnectPeers.restype = u32
 _lib.nrdCudaBarrier.argtypes = [C.c_void_p, C.c_void_p]
 _lib.nrdCudaBarrier.restype = u32
+_lib.nrdCudaRepartition.argtypes = [C.c_void_p, C.POINTER(u16), C.c_void_p]
+_lib.nrdCudaRepartition.restype = u32
 _lib.nrdCudaSynchronize.argtypes = [C.c_void_p, C.c_void_p]
 _lib.nrdCudaSynchronize.restype = u32
 _lib.nrdCudaSetTiming.argtypes = [C.c_void_p, C.c_int32]
@@ -390,6 +392,7 @@ class CudaContext(object):
         desc.device = device
         self.strip = (desc.stripY0, desc.stripY1)
         self.strip_height = strip_height
+        self.world_size = None  # set by connect_peers
         self.instance = instance
         self.width, self.height = width, height
         self._ctx = C.c_void_p()
@@ -457,9 +460,20 @@ class CudaContext(object):
             assert len(blob) == IPC_HANDLE_SIZE * world_size
             r = _lib.nrdCudaConnectPeers(self._ctx, rank, world_size, blob, None, starts)
         self._check("nrdCudaConnectPeers", r)
+        self.world_size = world_size
 
     def barrier(self, stream=0):
         self._check("nrdCudaBarrier", _lib.nrdCudaBarrier(self._ctx, C.c_void_p(stream)))
+
+    def repartition(self, strip_starts, stream=0):
+        """Collective between two frames: every connected rank passes the same world_size + 1 strip starts (include/nrd_b200.h).
+        Afterwards get_texture / copy address the new rows of this rank."""
+        if self.world_size is not None and len(strip_starts) != self.world_size + 1:  # the library reads world_size + 1 entries
+            raise ValueError("%d strip starts for a world of %d: give world_size + 1" % (len(strip_starts), self.world_size))
+        starts = (u16 * len(strip_starts))(*strip_starts)
+        self._check("nrdCudaRepartition", _lib.nrdCudaRepartition(self._ctx, starts, C.c_void_p(stream)))
+        viewz = self.get_texture(ResourceType.IN_VIEWZ)  # a full-resolution texture: its rows are the strip
+        self.strip = (viewz.firstRow, viewz.firstRow + viewz.rowsNum)
 
     def synchronize(self, stream=0):
         self._check("nrdCudaSynchronize", _lib.nrdCudaSynchronize(self._ctx, C.c_void_p(stream)))

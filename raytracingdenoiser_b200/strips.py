@@ -28,23 +28,33 @@ def partition_rows(height, world_size):
     return strip_height, strips
 
 
-def partition_rows_weighted(height, world_size, tile_row_cost, min_rows=TILE):
+def partition_rows_weighted(height, world_size, tile_row_cost, min_rows=TILE, max_rows=None):
     """Cost-balanced strips of whole 16-row tiles.  tile_row_cost[i] = estimated cost of tile row i (e.g. its number of
     non-sky tiles); returns (capacity, [(y0, y1)] per rank) with capacity = the tallest strip, to be passed as strip_height.
     Greedy prefix split: strip r ends at the first tile row where the running cost reaches (r + 1) / world_size of the total,
-    subject to every strip holding at least `min_rows` rows."""
+    subject to every strip holding at least `min_rows` rows and, if given, at most `max_rows` (the strip_height the contexts
+    reserved: a re-cut for nrdCudaRepartition).  Raises ValueError when no cut satisfies both."""
     tiles = (height + TILE - 1) // TILE
     cost = [float(c) for c in tile_row_cost]
     assert len(cost) == tiles, (len(cost), tiles)
     min_tiles = max(1, (min_rows + TILE - 1) // TILE)
     if min_tiles * world_size > tiles:
         raise ValueError("a %d-row frame cannot be cut into %d strips of at least %d rows" % (height, world_size, min_rows))
+    if max_rows is not None and (max_rows // TILE < min_tiles or max_rows // TILE * TILE * (world_size - 1) + max_rows < height):
+        raise ValueError("a %d-row frame cannot be cut into %d strips of %d to %d rows" % (height, world_size, min_rows, max_rows))
     total = sum(cost) or 1.0
     bounds, acc, t = [0], 0.0, 0
     for r in range(world_size - 1):
         target = total * (r + 1) / world_size
         lo = bounds[-1] + min_tiles                          # this strip needs min_tiles rows ...
         hi = tiles - min_tiles * (world_size - 1 - r)        # ... and so does every strip after it
+        if max_rows is not None:
+            max_tiles = max_rows // TILE
+            hi = min(hi, bounds[-1] + max_tiles)             # this strip fits max_rows ...
+            rest = max_tiles * TILE * (world_size - 2 - r) + max_rows
+            lo = max(lo, (height - rest + TILE - 1) // TILE)  # ... and so do the strips after it (the last may end mid-tile)
+            if lo > hi:
+                raise ValueError("a %d-row frame cannot be cut into %d strips of %d to %d rows" % (height, world_size, min_rows, max_rows))
         while t < lo or (t < hi and acc + 0.5 * cost[t] < target):
             acc += cost[t]
             t += 1
@@ -98,7 +108,20 @@ def exchange_ipc_handles(local_handle, group=None):
 
 
 class StripDenoiser(object):
-    """The strip of one rank: instance + strip-mode CUDA context.  IN_*/OUT_* strips live in the context's arena."""
+    """The strip of one rank: instance + strip-mode CUDA context.  IN_*/OUT_* strips live in the context's arena.
+
+    The strips can be re-cut between frames (repartition), keeping every history.  denoise() never does it by itself; a policy
+    for dynamic resolution, where every pass produces only the rows above tiles(max(rectSize.y, rectSizePrev.y)):
+
+        live = (max(rect_h, rect_h_prev) + 15) // 16                       # tile rows any pass of the frame produces
+        if live != last_live:                                               # the same decision on every rank
+            cost = [1.0 if t < live else 0.0 for t in range(tiles)]
+            _, cut = partition_rows_weighted(height, world, cost, min_rows=halo, max_rows=part.strip_height)
+            part.repartition(cut)                                           # before the frame's inputs are written
+            last_live = live
+
+    Reserve strip_height (the capacity) at creation for the most uneven cut wanted: the arena grows with it.  (REBLUR has a known
+    gap on frames where the rect grows, with or without re-cuts: DESIGN.md section 6, tests/test_gpu_strips_rect_growth.py.)"""
 
     def __init__(self, denoiser, width, height, rank, world_size, device=0, identifier=0, settings=None, halo_rows=None, partition=None):
         """partition = (capacity, [(y0, y1)] per rank) from partition_rows_weighted; default: uniform strips."""
@@ -123,6 +146,16 @@ class StripDenoiser(object):
     def connect_local(self, all_strips):
         """Single process (tests): every strip is a context of this process on a device that can address the others."""
         self.ctx.connect_peers(self.rank, self.world_size, arenas=[s.ctx.arena()[0] for s in all_strips], strip_starts=self.strip_starts)
+
+    def repartition(self, strips, stream=None):
+        """Collective between two frames (nrdCudaRepartition): every rank passes the same strips = [(y0, y1)] per rank, e.g. from
+        partition_rows_weighted(..., max_rows=self.strip_height).  set_inputs / read_outputs copy the new rows afterwards."""
+        if len(strips) != self.world_size or any(strips[r][1] != strips[r + 1][0] for r in range(self.world_size - 1)):
+            raise ValueError("strips must be %d contiguous (y0, y1) pairs: %r" % (self.world_size, strips))
+        starts = [y0 for y0, _ in strips] + [strips[-1][1]]
+        self.ctx.repartition(starts, self._stream(stream))
+        self.strip_starts = starts
+        self.y0, self.y1 = strips[self.rank]
 
     def _stream(self, stream):
         return stream.cuda_stream if stream is not None else torch.cuda.current_stream(self.device).cuda_stream
