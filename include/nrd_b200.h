@@ -377,6 +377,19 @@ NRD_API void nrdCudaDestroyContext(NrdCudaContext* context);
 // RGBA32_SFLOAT radiance / outputs, R16_SFLOAT viewZ, R16/R32_SFLOAT where R8_UNORM is listed.  The executor keeps a shadow copy in the listed format and converts around the passes (one extra streaming kernel per texture
 // and frame).  IN_NORMAL_ROUGHNESS must be the library's normal encoding (LibraryDesc).
 NRD_API nrd::Result nrdCudaSetUserTexture(NrdCudaContext* context, uint32_t resourceType, void* devicePtr, size_t pitchBytes, uint32_t format);
+// Binds a CUDA array (cudaArray_t / CUarray, level 0 of a mipmapped array, e.g. from
+// cudaExternalMemoryGetMappedMipmappedArray + cudaGetMipmappedArrayLevel) as an application texture: the way to reach a Vulkan /
+// D3D12 image with optimal tiling.  Formats as for nrdCudaSetUserTexture; texels are the raw bytes of `format`, so the array's
+// element size must be BytesPerTexel(format) (R10_G10_B10_A2_UNORM normals: a one-channel 32-bit array).  The array must be 2D (not
+// layered, not 3D), created with cudaArraySurfaceLoadStore, and at least resourceWidth x resourceHeight.  The executor keeps a
+// pitched shadow in the listed format: nrdCudaDenoise converts every array-bound input into it before the first pass and writes
+// every array-bound texture a pass of the frame wrote (outputs, IN_MV on a clear or a TemporalStabilization patch) back after the
+// last; nrdCudaExecuteDispatch converts what the dispatch reads before it and what it writes after it.  nrdCudaGetTexture /
+// UploadTexture / DownloadTexture act on the shadow.  Binding a type by array or by pointer replaces the previous binding of
+// either kind.  Refused: null context or array, or an array smaller than the resource size (INVALID_ARGUMENT); a layered / 3D
+// array, no surface load / store, a wrong element size or format, a resource type no supported denoiser uses, a strip-mode
+// context (UNSUPPORTED).
+NRD_API nrd::Result nrdCudaSetUserTextureArray(NrdCudaContext* context, uint32_t resourceType, void* cudaArray, uint32_t format);
 // Looks a texture up exactly like a DispatchDesc resource would be resolved.
 NRD_API nrd::Result nrdCudaGetTexture(NrdCudaContext* context, uint32_t resourceType, uint32_t indexInPool, NrdCudaTextureInfo* info);
 // Launches the kernel for one DispatchDesc on `stream` (cudaStream_t); the kernel produces the rows the context owns.  In strip

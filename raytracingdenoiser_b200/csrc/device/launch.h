@@ -3,6 +3,7 @@
 // (dispatch.cu) picks the family launcher from PassLaunch::kind, and the family launcher picks the kernel.
 #pragma once
 #include "common.cuh"
+#include "texel_convert.cuh"
 
 namespace nrdb200
 {
@@ -18,6 +19,8 @@ cudaError_t LaunchSigma(const PassLaunch& p);
 cudaError_t LaunchRelax(const PassLaunch& p);
 cudaError_t LaunchAux(const PassLaunch& p); // split-screen passes, REFERENCE denoiser
 cudaError_t LaunchPass(const PassLaunch& p); // cudaErrorNotSupported: the pass has no kernel
+// user textures bound as CUDA arrays (user_arrays.cu): array -> shadow (toShadow) or shadow -> array, every item in one launch
+cudaError_t LaunchArrayCopies(const ArrayCopyArgs& a, bool toShadow, cudaStream_t stream);
 
 #if !defined(NRD_B200_NO_STRIPS)
 // peer address table of one context slot, replicated into the constant memory of every kernel translation unit.
@@ -54,4 +57,5 @@ cudaError_t PreloadShiftedCopies(); // loads both kernels (see NRD_B200_LAUNCH: 
 namespace nrdb200_single
 {
 cudaError_t LaunchPass(const nrdb200_abi::PassLaunch& p);
+cudaError_t LaunchArrayCopies(const nrdb200_abi::ArrayCopyArgs& a, bool toShadow, cudaStream_t stream);
 }

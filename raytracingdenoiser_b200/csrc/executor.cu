@@ -113,18 +113,6 @@ struct ConvertArgs
     ConvertSide src, dst;
     int width, height;
 };
-__device__ __forceinline__ float LoadChannel(const uint8_t* texel, int kind, int ch)
-{
-    if (kind == 0) return (float)texel[ch] / 255.0f;
-    if (kind == 1) return __half2float(__ushort_as_half(((const unsigned short*)texel)[ch]));
-    return ((const float*)texel)[ch];
-}
-__device__ __forceinline__ void StoreChannel(uint8_t* texel, int kind, int ch, float v)
-{
-    if (kind == 0) texel[ch] = (unsigned char)__fadd_rn(__fmul_rn(__saturatef(v), 255.0f), 0.5f); // D3D float -> UNORM
-    else if (kind == 1) ((unsigned short*)texel)[ch] = __half_as_ushort(__float2half_rn(v));
-    else ((float*)texel)[ch] = v;
-}
 // channels the source does not have read 0 (a two-channel motion vector has no z / w), extra source channels are dropped
 __global__ void __launch_bounds__(256) ConvertFormatKernel(const __grid_constant__ ConvertArgs a)
 {
@@ -134,13 +122,30 @@ __global__ void __launch_bounds__(256) ConvertFormatKernel(const __grid_constant
     uint8_t* d = a.dst.texels + (size_t)y * a.dst.pitch + (size_t)x * a.dst.bytes;
     for (int ch = 0; ch < a.dst.channels; ch++) StoreChannel(d, a.dst.kind, ch, ch < a.src.channels ? LoadChannel(s, a.src.kind, ch) : 0.0f);
 }
+// The application's texture behind a shadow: a device pointer bound in a wider format (nrdCudaSetUserTexture), or a CUDA array
+// in any accepted format (nrdCudaSetUserTextureArray; converted by the kernels of device/user_arrays.cu).
 struct ForeignTexture
 {
-    void* ptr = nullptr;     // the application's texture
+    void* ptr = nullptr;     // pointer binding: the application's texture
     size_t pitch = 0;
+    bool isArray = false;    // array binding: the application's CUDA array, through a surface object created at bind time
+    cudaSurfaceObject_t surface = 0;
     Format format = Format::R8_UNORM;
     void* shadow = nullptr;  // cudaMalloc'ed copy in the kernels' format (NrdCudaContext::user[] points at it)
 };
+TexelFormat TexelFormatOf(Format f)
+{
+    FormatInfo info{};
+    ConvertibleFormat(f, info);
+    return {info.channels, info.kind, (int)BytesPerTexel(f)};
+}
+void ReleaseForeign(ForeignTexture& f)
+{
+    // an array binding always has a shadow: cudaFree waits for the device, so no conversion still uses the surface below
+    if (f.shadow) cudaFree(f.shadow);
+    if (f.isArray) cudaDestroySurfaceObject(f.surface);
+    f = ForeignTexture{};
+}
 
 struct NrdCudaContext
 {
@@ -176,6 +181,9 @@ struct NrdCudaContext
 
 namespace
 {
+// the refusal of both user-texture bindings on a strip-mode context
+constexpr const char* kStripUserTextures = "strip mode: user textures live in the context's arena, fill them through nrdCudaGetTexture / nrdCudaCopyTexture";
+
 Result Fail(NrdCudaContext* ctx, Result r, const std::string& msg)
 {
     if (ctx) ctx->lastError = msg;
@@ -302,6 +310,56 @@ Result UpdateRoughnessLut(NrdCudaContext* ctx, const float* hitDistParams, cudaS
     ctx->lutValid = true;
     return Result::SUCCESS;
 }
+
+// a zeroed shadow of user texture `type` in the kernels' format (ForeignTexture::shadow); on failure the type is left unbound
+Result AllocateShadow(NrdCudaContext* ctx, uint32_t type, Format format, size_t& pitch)
+{
+    ForeignTexture& f = ctx->foreign[type];
+    pitch = ((size_t)ctx->arena.desc.resourceWidth * BytesPerTexel(format) + 255) & ~(size_t)255;
+    if (cudaMalloc(&f.shadow, pitch * ctx->arena.desc.resourceHeight) != cudaSuccess)
+    {
+        f.shadow = nullptr;
+        ctx->user[type] = Texture{};
+        return Fail(ctx, Result::FAILURE, "cudaMalloc of the format-conversion shadow texture failed");
+    }
+    cudaMemset(f.shadow, 0, pitch * ctx->arena.desc.resourceHeight);
+    return Result::SUCCESS;
+}
+
+// The user textures in `types` (bit i = ResourceType i) that are bound as CUDA arrays, converted in one launch: array -> shadow
+// (toShadow) or shadow -> array, the whole resourceSize.  Pointer bindings are ConvertForeign's.
+Result ConvertArrays(NrdCudaContext* ctx, uint64_t types, bool toShadow, cudaStream_t stream)
+{
+    static_assert(std::size(kUserTextures) <= (size_t)kMaxArrayCopies && (size_t)ResourceType::MAX_NUM <= 64, "one launch, one bit per type");
+    ArrayCopyArgs a{};
+    for (const UserTexture& u : kUserTextures)
+    {
+        const ForeignTexture& f = ctx->foreign[(uint32_t)u.type];
+        if (!f.isArray || !((types >> (uint32_t)u.type) & 1u)) continue;
+        const Texture& t = ctx->user[(uint32_t)u.type];
+        a.items[a.n++] = {f.surface, (uint8_t*)t.ptr, t.pitch, TexelFormatOf(f.format), TexelFormatOf(t.format), (int)t.width, (int)t.height};
+    }
+    if (!a.n) return Result::SUCCESS;
+    // a one-GPU context that runs the strip build of the kernels (NRD_B200_FORCE_STRIP_KERNELS) runs its conversions there too
+    const cudaError_t e = ctx->forceStripKernels ? nrdb200::LaunchArrayCopies(a, toShadow, stream) : nrdb200_single::LaunchArrayCopies(a, toShadow, stream);
+    return e == cudaSuccess ? Result::SUCCESS : Fail(ctx, Result::FAILURE, std::string("CUDA array conversion: ") + cudaGetErrorString(e));
+}
+
+uint64_t Bit(ResourceType type) { return 1ull << (uint32_t)type; }
+
+// REBLUR / RELAX ClassifyTiles, the first pass of every frame, also decodes the guide surface from IN_NORMAL_ROUGHNESS, which
+// the dispatch does not bind (surf.h PassLaunch::guideNr)
+bool BuildsGuide(const PassKind& kind) { return (kind.family == Family::REBLUR || kind.family == Family::RELAX) && kind.pass == Pass::ClassifyTiles; }
+
+// the user textures some dispatch of `d[0, n)` binds as `binding`
+uint64_t TypesBoundAs(const DispatchDesc* d, uint32_t n, DescriptorType binding)
+{
+    uint64_t types = 0;
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t j = 0; j < d[i].resourcesNum; j++)
+            if (d[i].resources[j].descriptorType == binding && FindUserTexture(d[i].resources[j].type)) types |= Bit(d[i].resources[j].type);
+    return types;
+}
 } // namespace
 
 extern "C" {
@@ -366,8 +424,7 @@ NRD_API void nrdCudaDestroyContext(NrdCudaContext* ctx)
     if (ctx->roughnessLut) cudaFree(ctx->roughnessLut);
     if (ctx->roughnessLutStaging) cudaFreeHost(ctx->roughnessLutStaging);
     if (ctx->lutUploaded) cudaEventDestroy(ctx->lutUploaded);
-    for (ForeignTexture& f : ctx->foreign)
-        if (f.shadow) cudaFree(f.shadow);
+    for (ForeignTexture& f : ctx->foreign) ReleaseForeign(f);
     for (cudaEvent_t ev : ctx->timingEvents)
         if (ev) cudaEventDestroy(ev);
     delete ctx;
@@ -376,7 +433,7 @@ NRD_API void nrdCudaDestroyContext(NrdCudaContext* ctx)
 NRD_API Result nrdCudaSetUserTexture(NrdCudaContext* ctx, uint32_t resourceType, void* devicePtr, size_t pitchBytes, uint32_t format)
 {
     if (!ctx || resourceType >= (uint32_t)ResourceType::TRANSIENT_POOL || format >= (uint32_t)Format::MAX_NUM) return Result::INVALID_ARGUMENT;
-    if (ctx->arena.StripMode()) return Fail(ctx, Result::UNSUPPORTED, "strip mode: user textures live in the context's arena, fill them through nrdCudaGetTexture / nrdCudaCopyTexture");
+    if (ctx->arena.StripMode()) return Fail(ctx, Result::UNSUPPORTED, kStripUserTextures);
     const UserTexture* u = FindUserTexture((ResourceType)resourceType, Translucent(ctx->instance));
     if (!u) return Fail(ctx, Result::UNSUPPORTED, "resource type not consumed by the supported denoisers");
     const Format expected = u->format;
@@ -385,18 +442,12 @@ NRD_API Result nrdCudaSetUserTexture(NrdCudaContext* ctx, uint32_t resourceType,
     const bool wider = (Format)format != expected;
     if (wider && !WiderFormat(u->type, (Format)format, expected))
         return Fail(ctx, Result::UNSUPPORTED, "unsupported format for this resource type (see nrd_b200.h: the listed format, or a 16- / 32-bit float format with at least its channels)");
-    if (foreign.shadow) cudaFree(foreign.shadow); // (the previous binding of this resource type is replaced from here on)
-    foreign = ForeignTexture{};
+    ReleaseForeign(foreign); // (the previous binding of this resource type is replaced from here on)
     if (wider)
     {
-        const size_t shadowPitch = ((size_t)ctx->arena.desc.resourceWidth * BytesPerTexel(expected) + 255) & ~(size_t)255;
-        if (cudaMalloc(&foreign.shadow, shadowPitch * ctx->arena.desc.resourceHeight) != cudaSuccess)
-        {
-            foreign.shadow = nullptr;
-            ctx->user[resourceType] = Texture{};
-            return Fail(ctx, Result::FAILURE, "cudaMalloc of the format-conversion shadow texture failed");
-        }
-        cudaMemset(foreign.shadow, 0, shadowPitch * ctx->arena.desc.resourceHeight);
+        size_t shadowPitch = 0;
+        const Result r = AllocateShadow(ctx, resourceType, expected, shadowPitch);
+        if (r != Result::SUCCESS) return r;
         foreign.ptr = devicePtr;
         foreign.pitch = pitchBytes;
         foreign.format = (Format)format;
@@ -405,6 +456,64 @@ NRD_API Result nrdCudaSetUserTexture(NrdCudaContext* ctx, uint32_t resourceType,
     }
     ctx->user[resourceType] = ctx->arena.Describe(expected, 1, false, devicePtr, pitchBytes);
     return Result::SUCCESS;
+}
+
+NRD_API Result nrdCudaSetUserTextureArray(NrdCudaContext* ctx, uint32_t resourceType, void* cudaArray, uint32_t format)
+{
+    if (!ctx) return Result::INVALID_ARGUMENT;
+    if (!cudaArray) return Fail(ctx, Result::INVALID_ARGUMENT, "the CUDA array is null");
+    if (resourceType >= (uint32_t)ResourceType::TRANSIENT_POOL || format >= (uint32_t)Format::MAX_NUM) return Fail(ctx, Result::INVALID_ARGUMENT, "resource type or format out of range");
+    if (ctx->arena.StripMode()) return Fail(ctx, Result::UNSUPPORTED, kStripUserTextures);
+    const UserTexture* u = FindUserTexture((ResourceType)resourceType, Translucent(ctx->instance));
+    if (!u) return Fail(ctx, Result::UNSUPPORTED, "resource type not consumed by the supported denoisers");
+    const Format expected = u->format;
+    if ((Format)format != expected && !WiderFormat(u->type, (Format)format, expected))
+        return Fail(ctx, Result::UNSUPPORTED, "unsupported format for this resource type (see nrd_b200.h: the listed format, or a 16- / 32-bit float format with at least its channels)");
+    cudaChannelFormatDesc cd{};
+    cudaExtent extent{};
+    unsigned flags = 0;
+    cudaError_t e = cudaArrayGetInfo(&cd, &extent, &flags, (cudaArray_t)cudaArray);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError(); // not sticky: keep it from being reported by the next launch check
+        return Fail(ctx, Result::INVALID_ARGUMENT, std::string("cudaArrayGetInfo: ") + cudaGetErrorString(e));
+    }
+    if ((flags & (cudaArrayLayered | cudaArrayCubemap)) || extent.depth != 0)
+        return Fail(ctx, Result::UNSUPPORTED, "a layered, cube map or 3D CUDA array: bind a 2D array (level 0 of a mipmapped array)");
+    if (!(flags & cudaArraySurfaceLoadStore))
+        return Fail(ctx, Result::UNSUPPORTED, "the CUDA array was created without cudaArraySurfaceLoadStore (CUDA_ARRAY3D_SURFACE_LDST): the executor converts it through a surface");
+    const uint32_t elementBytes = (uint32_t)(cd.x + cd.y + cd.z + cd.w) / 8;
+    if (elementBytes != BytesPerTexel((Format)format))
+        return Fail(ctx, Result::UNSUPPORTED, "the CUDA array's element size (" + std::to_string(elementBytes) + " bytes) differs from the bytes per texel of the format (" +
+                                                  std::to_string(BytesPerTexel((Format)format)) + ")");
+    if (extent.width < ctx->arena.desc.resourceWidth || extent.height < ctx->arena.desc.resourceHeight)
+        return Fail(ctx, Result::INVALID_ARGUMENT, "the CUDA array (" + std::to_string(extent.width) + " x " + std::to_string(extent.height) +
+                                                       ") is smaller than the context's resource size");
+    cudaResourceDesc rd{};
+    rd.resType = cudaResourceTypeArray;
+    rd.res.array.array = (cudaArray_t)cudaArray;
+    cudaSurfaceObject_t surface = 0;
+    e = cudaCreateSurfaceObject(&surface, &rd);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return Fail(ctx, Result::UNSUPPORTED, std::string("cudaCreateSurfaceObject: ") + cudaGetErrorString(e));
+    }
+    ForeignTexture& foreign = ctx->foreign[resourceType];
+    ReleaseForeign(foreign); // (the previous binding of this resource type is replaced from here on)
+    size_t shadowPitch = 0;
+    const Result r = AllocateShadow(ctx, resourceType, expected, shadowPitch);
+    if (r != Result::SUCCESS)
+    {
+        cudaDestroySurfaceObject(surface);
+        return r;
+    }
+    foreign.isArray = true;
+    foreign.surface = surface;
+    foreign.format = (Format)format;
+    ctx->user[resourceType] = ctx->arena.Describe(expected, 1, false, foreign.shadow, shadowPitch);
+    // the shadow starts as the array: texels no pass writes (outside the rect) go back to the array as the application left them
+    return ConvertArrays(ctx, Bit((ResourceType)resourceType), true, nullptr);
 }
 
 NRD_API Result nrdCudaGetTexture(NrdCudaContext* ctx, uint32_t resourceType, uint32_t indexInPool, NrdCudaTextureInfo* info)
@@ -459,7 +568,7 @@ namespace
 Result ConvertForeign(NrdCudaContext* ctx, ResourceType type, bool toNative, cudaStream_t stream)
 {
     const ForeignTexture& f = ctx->foreign[(uint32_t)type];
-    if (!f.shadow) return Result::SUCCESS;
+    if (!f.shadow || f.isArray) return Result::SUCCESS;
     const Texture& t = ctx->user[(uint32_t)type];
     const ConvertSide app = Side(f.ptr, f.pitch, f.format), native = Side(t.ptr, t.pitch, t.format);
     const ConvertArgs a{toNative ? app : native, toNative ? native : app, t.width, t.height};
@@ -487,7 +596,11 @@ Result ConvertBound(NrdCudaContext* ctx, const DispatchDesc* d, DescriptorType b
             const Result r = ConvertForeign(ctx, d->resources[i].type, binding == DescriptorType::TEXTURE, stream);
             if (r != Result::SUCCESS) return r;
         }
-    return Result::SUCCESS;
+    uint64_t types = TypesBoundAs(d, 1, binding);
+    const Scheduler* scheduler = (const Scheduler*)ctx->instance;
+    if (binding == DescriptorType::TEXTURE && d->pipelineIndex < GetInstanceDesc(*ctx->instance).pipelinesNum && BuildsGuide(scheduler->PipelineKind(d->pipelineIndex)))
+        types |= Bit(ResourceType::IN_NORMAL_ROUGHNESS);
+    return ConvertArrays(ctx, types, binding == DescriptorType::TEXTURE, stream);
 }
 
 // After the barrier of a pass that wrote staged guide inputs (REBLUR TemporalStabilization with isBaseColorMetalnessAvailable
@@ -567,7 +680,7 @@ Result ExecuteInternal(NrdCudaContext* ctx, const DispatchDesc* d, void* stream,
     // accumulation slows down on resolved pixels; RELAX and the split-screen passes reject them in their launchers
     // decoded-guide surface: ClassifyTiles (first pass of every REBLUR frame) fills it, all later passes of the frame read it
     const bool isReblur = kind.family == Family::REBLUR, isRelax = kind.family == Family::RELAX, isClear = kind.family == Family::CLEAR;
-    const bool buildsGuide = (isReblur || isRelax) && kind.pass == Pass::ClassifyTiles;
+    const bool buildsGuide = BuildsGuide(kind);
     const bool isSplitScreen = kind.pass == Pass::SplitScreen; // may be the only pass of the frame (splitScreen >= 1)
     const bool readsGuide = (isReblur || isRelax) && !buildsGuide && !isSplitScreen; // every other REBLUR / RELAX pass reads it (REBLUR: and the roughness table)
     p.guide = ctx->arena.ToSurf(ctx->guide);
@@ -731,6 +844,10 @@ NRD_API Result nrdCudaDenoise(NrdCudaContext* ctx, const Identifier* identifiers
     Result r = GetComputeDispatches(*ctx->instance, identifiers, identifiersNum, dispatches, n);
     if (r != Result::SUCCESS) return r;
     r = ConvertForeignAll(ctx, true, (cudaStream_t)stream); // inputs bound in a wider format -> the kernels' format
+    uint64_t inputs = 0;
+    for (const UserTexture& u : kUserTextures)
+        if (u.isInput) inputs |= Bit(u.type);
+    if (r == Result::SUCCESS) r = ConvertArrays(ctx, inputs, true, (cudaStream_t)stream); // inputs bound as CUDA arrays -> their shadows
     if (r != Result::SUCCESS) return r;
     r = FrameStart(ctx, stream);
     if (r != Result::SUCCESS) return r;
@@ -740,6 +857,9 @@ NRD_API Result nrdCudaDenoise(NrdCudaContext* ctx, const Identifier* identifiers
         if (r != Result::SUCCESS) return r;
     }
     r = ConvertForeignAll(ctx, false, (cudaStream_t)stream); // outputs -> the application's wider format
+    // every user texture some pass of the frame wrote -> its CUDA array: the outputs, and IN_MV when the frame-0 clear zeroes it or
+    // REBLUR TemporalStabilization patches it, so that the array ends the frame as a pointer-bound texture would
+    if (r == Result::SUCCESS) r = ConvertArrays(ctx, TypesBoundAs(dispatches, n, DescriptorType::STORAGE_TEXTURE), false, (cudaStream_t)stream);
     if (r != Result::SUCCESS) return r;
     if (launches) *launches = n;
     return Result::SUCCESS;

@@ -218,6 +218,8 @@ _lib.nrdCudaDestroyContext.argtypes = [C.c_void_p]
 _lib.nrdCudaDestroyContext.restype = None
 _lib.nrdCudaSetUserTexture.argtypes = [C.c_void_p, u32, C.c_void_p, C.c_size_t, u32]
 _lib.nrdCudaSetUserTexture.restype = u32
+_lib.nrdCudaSetUserTextureArray.argtypes = [C.c_void_p, u32, C.c_void_p, u32]
+_lib.nrdCudaSetUserTextureArray.restype = u32
 _lib.nrdCudaGetTexture.argtypes = [C.c_void_p, u32, u32, C.POINTER(NrdCudaTextureInfo)]
 _lib.nrdCudaGetTexture.restype = u32
 _lib.nrdCudaExecuteDispatch.argtypes = [C.c_void_p, C.POINTER(DispatchDesc), C.c_void_p]
@@ -254,7 +256,7 @@ IPC_HANDLE_SIZE = 64
 
 EXPORTED_SYMBOLS = ["CreateInstance", "DestroyInstance", "GetLibraryDesc", "GetInstanceDesc", "SetCommonSettings", "SetDenoiserSettings",
                     "GetComputeDispatches", "GetResourceTypeString", "GetDenoiserString", "nrdCudaCreateContext", "nrdCudaDestroyContext",
-                    "nrdCudaSetUserTexture", "nrdCudaGetTexture", "nrdCudaExecuteDispatch", "nrdCudaDenoise", "nrdCudaUploadTexture", "nrdCudaDownloadTexture", "nrdCudaGetLastError", "nrdCudaGetLaunchCount",
+                    "nrdCudaSetUserTexture", "nrdCudaSetUserTextureArray", "nrdCudaGetTexture", "nrdCudaExecuteDispatch", "nrdCudaDenoise", "nrdCudaUploadTexture", "nrdCudaDownloadTexture", "nrdCudaGetLastError", "nrdCudaGetLaunchCount",
                     "nrdCudaCopyTexture", "nrdCudaGetArena", "nrdCudaGetIpcHandle", "nrdCudaConnectPeers", "nrdCudaBarrier", "nrdCudaSynchronize", "nrdCudaSetTiming", "nrdCudaGetTiming"]
 
 
@@ -380,7 +382,7 @@ class Instance(object):
 
 
 class CudaContext(object):
-    """CUDA executor for one Instance (replaces nrd::Integration).  Textures are plain device pointers + pitch."""
+    """CUDA executor for one Instance (replaces nrd::Integration).  Textures are plain device pointers + pitch, or CUDA arrays."""
 
     def __init__(self, instance, width, height, device=0, strip=None, strip_height=0, halo_rows=0):
         """strip=(y0, y1), strip_height=S, halo_rows=H: strip-mode context of a multi-GPU run (see include/nrd_b200.h)."""
@@ -420,6 +422,12 @@ class CudaContext(object):
     def set_user_texture(self, resource_type, device_ptr, pitch_bytes, fmt):
         self._check("nrdCudaSetUserTexture(%s)" % ResourceType(resource_type).name,
                     _lib.nrdCudaSetUserTexture(self._ctx, int(resource_type), C.c_void_p(device_ptr), pitch_bytes, int(fmt)))
+
+    def set_user_texture_array(self, resource_type, array_handle, fmt):
+        """array_handle: a cudaArray_t / CUarray as an int (level 0 of a mipmapped array, e.g. an imported Vulkan / D3D12 image)
+        created with surface load / store; the executor converts it to and from a shadow in the kernels' format around the passes."""
+        self._check("nrdCudaSetUserTextureArray(%s)" % ResourceType(resource_type).name,
+                    _lib.nrdCudaSetUserTextureArray(self._ctx, int(resource_type), C.c_void_p(array_handle), int(fmt)))
 
     def get_texture(self, resource_type, index_in_pool=0):
         info = NrdCudaTextureInfo()
